@@ -39,14 +39,8 @@ struct Events {
     ~Events() { cudaEventDestroy(a); cudaEventDestroy(b); }
 };
 
-// Band-width classes, one launch per class. Up to 1024 offsets the register-resident wavefront kernel runs with
-// C = offsets/64 per sub-chunk (no shared memory); wider bands use the shared-memory scan kernel (C = 0).
-struct DpClass { uint32_t wMax; int c; };
-const DpClass kClasses[] = {{64, 1}, {128, 2}, {192, 3}, {256, 4}, {384, 6}, {512, 8}, {768, 12}, {1024, 16},
-                            {2048, 0}, {4096, 0}, {8192, 0}, {16384, 0}};
-constexpr int kClassCount = 12;
-constexpr uint32_t kMaxBandWidth = 16384;
-
+// One launch per band class (dpClassAt). Wavefront classes run on groups of lanes in blocks of kDpMaxWarpsPerBlock
+// warps, with no shared memory; the scan kernel (c = 0) takes as many warps as fit its shared memory.
 uint32_t warpsForClass(const DpClass& k)
 {
     if(k.c > 0) return kDpMaxWarpsPerBlock;
@@ -61,54 +55,51 @@ size_t smemForClass(const DpClass& k, uint32_t warps) { return k.c > 0 ? 0 : siz
 size_t scanKernelSmemLimit()
 {
     size_t most = 0;
-    for(const DpClass& k : kClasses) most = std::max(most, smemForClass(k, warpsForClass(k)));
+    for(uint32_t k = 0; k < kDpClassCount; k++) most = std::max(most, smemForClass(dpClassAt(k), warpsForClass(dpClassAt(k))));
     return most;
 }
+constexpr uint32_t kMaxBandWidth = dpClassAt(kDpClassCount - 1).wMax;
+// Launch geometry of a class: blocks of `warps` warps, 32 / lanes jobs per warp.
+struct DpLaunch { uint32_t blocks, threads; size_t smem; };
+DpLaunch dpLaunch(const DpClass& k, uint32_t jobs)
+{
+    const uint32_t warps = warpsForClass(k);
+    return DpLaunch{ceilDiv(jobs, warps * (32 / k.lanes)), warps * 32, smemForClass(k, warps)};
+}
 
-template<class... Args> void launchStage1(const DpClass& k, uint32_t blocks, uint32_t threads, size_t smem, cudaStream_t st, Args... args)
+// Stage 1 with a trace / stage 2: the kernel instantiation of band class k.
+template<uint32_t K = 0, class... Args> void launchStage1(uint32_t k, const DpLaunch& l, cudaStream_t st, Args... args)
 {
-    switch(k.c) {
-    case 1: SHB_LAUNCH(method3Stage1Kernel<1>, blocks, threads, smem, st, args...); break;
-    case 2: SHB_LAUNCH(method3Stage1Kernel<2>, blocks, threads, smem, st, args...); break;
-    case 3: SHB_LAUNCH(method3Stage1Kernel<3>, blocks, threads, smem, st, args...); break;
-    case 4: SHB_LAUNCH(method3Stage1Kernel<4>, blocks, threads, smem, st, args...); break;
-    case 6: SHB_LAUNCH(method3Stage1Kernel<6>, blocks, threads, smem, st, args...); break;
-    case 8: SHB_LAUNCH(method3Stage1Kernel<8>, blocks, threads, smem, st, args...); break;
-    case 12: SHB_LAUNCH(method3Stage1Kernel<12>, blocks, threads, smem, st, args...); break;
-    case 16: SHB_LAUNCH(method3Stage1Kernel<16>, blocks, threads, smem, st, args...); break;
-    default:
-        SHB_CUDA(cudaFuncSetAttribute(method3Stage1Kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(scanKernelSmemLimit())));
-        SHB_LAUNCH(method3Stage1Kernel<0>, blocks, threads, smem, st, args...); break;
+    if constexpr(K < kDpClassCount) {
+        if(k != K) { launchStage1<K + 1>(k, l, st, args...); return; }
+        constexpr DpClass cl = dpClassAt(K);
+        if constexpr(cl.c == 0) {
+            SHB_CUDA(cudaFuncSetAttribute(method3Stage1Kernel<32, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(scanKernelSmemLimit())));
+        }
+        auto* kernel = &method3Stage1Kernel<int(cl.lanes), int(cl.c)>;
+        SHB_LAUNCH(kernel, l.blocks, l.threads, l.smem, st, args...);
     }
 }
-// Stage 1 of method 3 for downsampled reads of at most 32*R markers (rows per lane R).
-const int kForwardRows[] = {2, 4, 6, 8, 12, 16};
-constexpr int kForwardClassCount = 6;        // row limits 64 .. 512 = kClasses[0..5].wMax
-template<class... Args> void launchStage1Forward(int rows, uint32_t blocks, uint32_t threads, cudaStream_t st, Args... args)
+template<uint32_t K = 0, class... Args> void launchBanded(uint32_t k, const DpLaunch& l, cudaStream_t st, Args... args)
 {
-    switch(rows) {
-    case 2: SHB_LAUNCH(method3Stage1ForwardKernel<2>, blocks, threads, 0, st, args...); break;
-    case 4: SHB_LAUNCH(method3Stage1ForwardKernel<4>, blocks, threads, 0, st, args...); break;
-    case 6: SHB_LAUNCH(method3Stage1ForwardKernel<6>, blocks, threads, 0, st, args...); break;
-    case 8: SHB_LAUNCH(method3Stage1ForwardKernel<8>, blocks, threads, 0, st, args...); break;
-    case 12: SHB_LAUNCH(method3Stage1ForwardKernel<12>, blocks, threads, 0, st, args...); break;
-    default: SHB_LAUNCH(method3Stage1ForwardKernel<16>, blocks, threads, 0, st, args...); break;
+    if constexpr(K < kDpClassCount) {
+        if(k != K) { launchBanded<K + 1>(k, l, st, args...); return; }
+        constexpr DpClass cl = dpClassAt(K);
+        if constexpr(cl.c == 0) {
+            SHB_CUDA(cudaFuncSetAttribute(bandedAlignKernel<32, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(scanKernelSmemLimit())));
+        }
+        auto* kernel = &bandedAlignKernel<int(cl.lanes), int(cl.c)>;
+        SHB_LAUNCH(kernel, l.blocks, l.threads, l.smem, st, args...);
     }
 }
-template<class... Args> void launchBanded(const DpClass& k, uint32_t blocks, uint32_t threads, size_t smem, cudaStream_t st, Args... args)
+// Stage 1 of method 3 without a trace (downsampled reads of at most 512 markers): forward class k.
+template<uint32_t K = 0, class... Args> void launchStage1Forward(uint32_t k, uint32_t jobs, cudaStream_t st, Args... args)
 {
-    switch(k.c) {
-    case 1: SHB_LAUNCH(bandedAlignKernel<1>, blocks, threads, smem, st, args...); break;
-    case 2: SHB_LAUNCH(bandedAlignKernel<2>, blocks, threads, smem, st, args...); break;
-    case 3: SHB_LAUNCH(bandedAlignKernel<3>, blocks, threads, smem, st, args...); break;
-    case 4: SHB_LAUNCH(bandedAlignKernel<4>, blocks, threads, smem, st, args...); break;
-    case 6: SHB_LAUNCH(bandedAlignKernel<6>, blocks, threads, smem, st, args...); break;
-    case 8: SHB_LAUNCH(bandedAlignKernel<8>, blocks, threads, smem, st, args...); break;
-    case 12: SHB_LAUNCH(bandedAlignKernel<12>, blocks, threads, smem, st, args...); break;
-    case 16: SHB_LAUNCH(bandedAlignKernel<16>, blocks, threads, smem, st, args...); break;
-    default:
-        SHB_CUDA(cudaFuncSetAttribute(bandedAlignKernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(scanKernelSmemLimit())));
-        SHB_LAUNCH(bandedAlignKernel<0>, blocks, threads, smem, st, args...); break;
+    if constexpr(K < kDpForwardClassCount) {
+        if(k != K) { launchStage1Forward<K + 1>(k, jobs, st, args...); return; }
+        constexpr DpForwardClass f = dpForwardClassAt(K);
+        auto* kernel = &method3Stage1ForwardKernel<int(f.lanes), int(f.rows)>;
+        SHB_LAUNCH(kernel, ceilDiv(jobs, kDpMaxWarpsPerBlock * (32 / f.lanes)), kDpMaxWarpsPerBlock * 32, 0, st, args...);
     }
 }
 
@@ -127,7 +118,7 @@ struct Batch {
     DeviceBuffer<uint8_t> gridFlags;
     DeviceBuffer<int32_t> gridBands;
     // band-class ordering of the DP jobs
-    DeviceBuffer<uint32_t> classLimits, orderValsA, orderValsB;
+    DeviceBuffer<uint32_t> orderValsA, orderValsB;
     DeviceBuffer<uint64_t> orderKeysA, orderKeysB;
     const uint32_t* order = nullptr;
 };
@@ -404,22 +395,14 @@ void copyToHostPipelined(shb_context* c, void* dstHost, const void* srcDevice, u
 
 // Groups the runnable jobs by band class (longest first inside a class). Returns per-class counts; b.order holds the
 // job indices, class after class.
-void buildClassOrder(AlignWorker& w, const DpJob* jobs, uint32_t nJobs, std::vector<uint64_t>& classCounts, uint32_t forwardClasses = 0)
+void buildClassOrder(AlignWorker& w, const DpJob* jobs, uint32_t nJobs, std::vector<uint64_t>& classCounts, bool forward = false)
 {
     cudaStream_t st = w.stream;
     Batch& b = w.batch;
-    classCounts.assign(kClassCount + forwardClasses, 0);
+    classCounts.assign(kDpClassCount + (forward ? kDpForwardClassCount : 0), 0);
     if(nJobs == 0) return;
-    if(!b.classLimits.get()) {
-        b.classLimits.reserve(kClassCount);
-        uint32_t limits[kClassCount];
-        for(int k = 0; k < kClassCount; k++) limits[k] = kClasses[k].wMax;
-        SHB_CUDA(cudaMemcpyAsync(b.classLimits.get(), limits, sizeof(limits), cudaMemcpyHostToDevice, st));
-        SHB_CUDA(cudaStreamSynchronize(st));
-    }
     b.orderKeysA.reserve(nJobs); b.orderKeysB.reserve(nJobs); b.orderValsA.reserve(nJobs); b.orderValsB.reserve(nJobs);
-    SHB_LAUNCH(dpClassKeysKernel, ceilDiv(nJobs, 256), 256, 0, st, jobs, nJobs, (const uint32_t*)b.classLimits.get(), uint32_t(kClassCount),
-               forwardClasses, b.orderKeysA.get(), b.orderValsA.get());
+    SHB_LAUNCH(dpClassKeysKernel, ceilDiv(nJobs, 256), 256, 0, st, jobs, nJobs, forward, b.orderKeysA.get(), b.orderValsA.get());
     const int ranges[1][2] = {{0, kDpLengthKeyBits + kDpClassKeyBits}};
     const bool inB = radixSort<true>(b.orderKeysA.get(), b.orderKeysB.get(), b.orderValsA.get(), b.orderValsB.get(), nJobs, ranges, 1, w.sortWs, st);
     b.order = inB ? b.orderValsB.get() : b.orderValsA.get();
@@ -461,11 +444,9 @@ void runBandedJobs(AlignWorker& w, uint32_t nJobs, const uint32_t* sequences, Dp
     // on a high-priority stream.
     size_t unit = 0;
     forEachClassConcurrently(w, classCounts, envCount("SHB_ALIGN_CHUNK", 32768), [&](int k, uint32_t count, uint64_t offset, cudaStream_t s) {
-        const uint32_t warps = warpsForClass(kClasses[k]);
-        const size_t smem = smemForClass(kClasses[k], warps);
         BandedArgs gk = g;
-        gk.n = count; gk.order = b.order + offset; gk.wMax = kClasses[k].wMax;
-        launchBanded(kClasses[k], ceilDiv(count, warps), warps * 32, smem, s, gk, (const DpJob*)b.jobs.get(), b.trace.get(), b.endCells.get());
+        gk.n = count; gk.order = b.order + offset; gk.wMax = dpClassAt(k).wMax;
+        launchBanded(uint32_t(k), dpLaunch(dpClassAt(k), count), s, gk, (const DpJob*)b.jobs.get(), b.trace.get(), b.endCells.get());
         if(unit == w.unitEvents.size()) {
             cudaEvent_t e = nullptr;
             SHB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -630,22 +611,19 @@ void processBatch(AlignCall& call, AlignWorker& w, uint64_t begin, uint32_t nb, 
             g1.toc = c->toc.get(); g1.dsToc = ac.dsToc.get(); g1.dsKmer = ac.dsKmer.get(); g1.dsOrdinal = ac.dsOrdinal.get();
             g1.scores = call.scores; g1.fma = FmaUnits{1, 2, 4}; g1.bandExtend = o.bandExtend; g1.maxBand = o.maxBand;
             std::vector<uint64_t> classCounts1;
-            buildClassOrder(w, b.jobs1.get(), nb, classCounts1, kForwardClassCount);
+            buildClassOrder(w, b.jobs1.get(), nb, classCounts1, true);
             SHB_CUDA(cudaEventRecord(w.dp1a, st));
             forEachClassConcurrently(w, classCounts1, 0xffffffffu, [&](int k, uint32_t count, uint64_t offset, cudaStream_t s) {
                 Method3Args gk = g1;
                 gk.n = count; gk.order = b.order + offset;
-                if(k < kForwardClassCount) {
+                if(uint32_t(k) < kDpForwardClassCount) {
                     gk.wMax = 0;
-                    launchStage1Forward(kForwardRows[k], ceilDiv(count, kDpMaxWarpsPerBlock), kDpMaxWarpsPerBlock * 32, s, gk,
-                                        (const DpJob*)b.jobs1.get(), b.jobs.get());
+                    launchStage1Forward(uint32_t(k), count, s, gk, (const DpJob*)b.jobs1.get(), b.jobs.get());
                     return;
                 }
-                const DpClass& cls = kClasses[k - kForwardClassCount];      // too long for the forward kernel: DP with a trace
-                const uint32_t warps = warpsForClass(cls);
-                const size_t smem = smemForClass(cls, warps);
-                gk.wMax = cls.wMax;
-                launchStage1(cls, ceilDiv(count, warps), warps * 32, smem, s, gk, b.jobs1.get(), b.trace.get(), b.jobs.get(), b.ordinals.get());
+                const uint32_t cls = uint32_t(k) - kDpForwardClassCount;   // too long for the forward kernel: DP with a trace
+                gk.wMax = dpClassAt(cls).wMax;
+                launchStage1(cls, dpLaunch(dpClassAt(cls), count), s, gk, b.jobs1.get(), b.trace.get(), b.jobs.get(), b.ordinals.get());
             });
             SHB_CUDA(cudaEventRecord(w.dp1b, st));
             stage1Timed = true;

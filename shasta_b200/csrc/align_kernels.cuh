@@ -123,12 +123,35 @@ constexpr int32_t kEndCellNone = SHB_DP_END_FIRST_MAX ? 0x7fffffff : -1;        
 
 // Physical band layout of the wavefront kernels: band offset e = j - i + hi in [0, W) sits at physical offset p = e + 1;
 // p = 0 and p = W + 1 are BARRIER offsets whose gap score is "minus infinity", so that nothing flows around the band
-// edges; physical offsets beyond W + 1 are padding that only the barrier ever reads. Width classes are multiples of 64.
-__host__ __device__ inline uint32_t dpPaddedWidth(int32_t lo, int32_t hi) { return (uint32_t(hi - lo + 1) + 2u + 63u) & ~63u; }
+// edges; physical offsets beyond W + 1 are padding that only the barrier ever reads.
+//
+// Band classes, one launch each. A wavefront class (c > 0) runs a job on a group of `lanes` lanes, each owning two
+// sub-chunks of c physical offsets, so it holds W + 2 <= wMax = 2 * lanes * c. Narrow bands run on groups of 8 lanes
+// (four jobs per warp, widths 32, 48, ..., 128), wider ones on a whole warp; c = 0 is the shared-memory scan kernel.
+// The padded width of a job (its trace row length) is W + 2 rounded up to 2 * lanes.
+struct DpClass { uint32_t wMax, lanes, c; };
+constexpr uint32_t kDpClassCount = 17, kDpGroupClassCount = 7;
+__host__ __device__ constexpr DpClass dpClassAt(uint32_t k)
+{
+    const uint32_t m = k - kDpGroupClassCount;                          // whole-warp classes: c = 3, 4, 6, 8, 12, 16
+    const uint32_t warpC = m < 2 ? m + 3u : m < 4 ? 2u * m + 2u : 4u * m - 4u;
+    return k < kDpGroupClassCount ? DpClass{16u * (k + 2u), 8u, k + 2u}
+         : m < 6 ? DpClass{64u * warpC, 32u, warpC}
+         : DpClass{2048u << (m - 6u), 32u, 0u};
+}
+struct DpShape { uint32_t cls, lanes, c, wpad; };
+// The class of a band lo..hi (the last class, with a padded width beyond its wMax, for bands too wide for any).
+__host__ __device__ inline DpShape dpBandShape(int32_t lo, int32_t hi)
+{
+    const uint32_t need = uint32_t(hi - lo + 1) + 2u;
+    uint32_t k = 0;
+    while(k + 1 < kDpClassCount && need > dpClassAt(k).wMax) k++;
+    const DpClass cl = dpClassAt(k);
+    return DpShape{k, cl.lanes, cl.c, (need + 2u * cl.lanes - 1u) & ~(2u * cl.lanes - 1u)};
+}
 constexpr int32_t kGapBarrier = -(1 << 28);
 // Columns of the matrix that hold at least one in-band cell: max(0, lo) <= i <= min(nx, ny + hi). The wavefront kernel
 // only visits these (a band that enters through the top edge or leaves through the bottom edge skips the rest).
-constexpr uint32_t kDpWavefrontMaxWidth = 1024;
 __host__ __device__ inline int32_t dpFirstColumn(int32_t lo) { return lo > 0 ? lo : 0; }
 __host__ __device__ inline int32_t dpLastColumn(uint32_t nx, uint32_t ny, int32_t hi)
 {
@@ -137,13 +160,14 @@ __host__ __device__ inline int32_t dpLastColumn(uint32_t nx, uint32_t ny, int32_
 }
 __host__ __device__ inline uint64_t dpTraceWords(uint32_t nx, uint32_t ny, int32_t lo, int32_t hi)
 {
-    const uint32_t Wpad = dpPaddedWidth(lo, hi);
+    const DpShape s = dpBandShape(lo, hi);
     uint64_t columns = nx;                                              // scan kernel: by-column layout over all columns
-    if(Wpad <= kDpWavefrontMaxWidth) {
+    if(s.c) {
         const int64_t active = int64_t(dpLastColumn(nx, ny, hi)) - dpFirstColumn(lo);
         columns = uint64_t(active > 0 ? active : 0);
     }
-    return ((columns + 31u) / 16u + 2u) * Wpad;                         // rows of the by-step layout (+1 spare row)
+    // Rows of the by-step layout: columns + 1 steps plus the lane skew, and one spare row that the traceback may read.
+    return ((columns + s.lanes + 15u) / 16u + 1u) * s.wpad;
 }
 
 // Warp-cooperative banded overlap DP. Band offset e = j - i + hi in [0, W). Lanes own e % 32.
@@ -160,7 +184,7 @@ __device__ inline void bandedOverlapDp(const uint32_t* __restrict__ a, uint32_t 
 {
     const unsigned lane = threadIdx.x & 31u;
     const int32_t W = hi - lo + 1;
-    const int32_t Wpad = int32_t(dpPaddedWidth(lo, hi));
+    const int32_t Wpad = int32_t(dpBandShape(lo, hi).wpad);
     const int32_t chunks = Wpad >> 5;
 
     bestScore = kNegInf * 2; bestI = -1; bestJ = -1;
@@ -239,9 +263,10 @@ __device__ inline void bandedOverlapDp(const uint32_t* __restrict__ a, uint32_t 
 }
 
 // ---------------------------------------------------------------------------------------------
-// Register-resident wavefront version of the same DP for bands of up to 64*C - 2 offsets (C <= 16).
-// The 64*C PHYSICAL offsets (band offset e at p = e + 1, barriers at p = 0 and p = W + 1, see dpPaddedWidth) are cut into
-// 64 sub-chunks of C consecutive offsets; lane l owns sub-chunks 2l ("A") and 2l+1 ("B"). Cell (i, p) depends on (i-1, p),
+// Register-resident wavefront version of the same DP for bands of up to 2*G*C - 2 offsets, run by a group of G lanes
+// (G = 8 or 32, C <= 16). The 2*G*C PHYSICAL offsets (band offset e at p = e + 1, barriers at p = 0 and p = W + 1, see
+// dpBandShape) are cut into 2G sub-chunks of C consecutive offsets; lane l of the group owns sub-chunks 2l ("A") and
+// 2l+1 ("B"). Cell (i, p) depends on (i-1, p),
 // (i-1, p+1) and (i, p-1), so sub-chunk s can process column i at step T = 2i + s: on even steps every lane advances its A
 // sub-chunk, on odd steps its B sub-chunk (no divergence, every lane busy every step), and the only inter-lane traffic is
 // one shuffle per half-step (the neighbouring sub-chunk's boundary score). All scores of the previous column live in
@@ -254,7 +279,7 @@ __device__ inline void bandedOverlapDp(const uint32_t* __restrict__ a, uint32_t 
 // (i == 0 or j == 0, score 0). gap = the gap score, or kGapBarrier for the two barrier offsets: a barrier cell can only
 // be entered by a gap move, so its score is "minus infinity" plus something bounded, whatever its neighbours hold, and
 // no finite score ever passes through it; no per-cell clamp and no special case for the first / last lane is needed
-// (lane 0's first offset and lane 31's last offset are barrier or padding, so the values their shuffles wrap around
+// (lane 0's first offset and lane G-1's last offset are barrier or padding, so the values their shuffles wrap around
 // are never used by an in-band cell).
 template<int C> struct SubChunkLimits { int32_t first[C]; int32_t gap[C]; };
 
@@ -270,7 +295,7 @@ template<int C> __device__ __forceinline__ void initSubChunkLimits(SubChunkLimit
 
 // Trace layout of the wavefront kernel: the codes are stored by STEP, not by column. Lane l works on column
 // i = t2 - l in step t2, and every lane stores the codes of its last 16 steps in the same step (t2 % 16 == 15), so the
-// stores are warp-uniform and fully coalesced: word (t2 >> 4) * Wpad + p holds, at bits 2*(t2 % 16), the code of cell
+// stores are group-uniform and coalesced: word (t2 >> 4) * Wpad + p holds, at bits 2*(t2 % 16), the code of cell
 // (t2 - p / (2C), p). The traceback re-aligns two such words into a by-column word with one funnel shift.
 
 // One sub-chunk (C consecutive physical offsets) of column i. Straight-line code for the common interior cell; cells
@@ -282,6 +307,8 @@ template<int C> __device__ __forceinline__ void initSubChunkLimits(SubChunkLimit
 // the recurrence and the trace bookkeeping are therefore written as integer multiply-adds with run-time multipliers
 // (a kernel argument the compiler cannot fold): IMAD issues on the FMA pipe. FmaUnits = {1, 2, 4}.
 struct FmaUnits { int32_t one, two, four; };
+// Sub-chunk widths up to this one run their 16-step blocks fully unrolled, with the trace codes added in place.
+constexpr int kDpInPlaceTraceMaxC = 4;
 __device__ __forceinline__ int32_t fmaPipeAdd(int32_t a, int32_t b, int32_t one)
 {
     int32_t r;
@@ -380,7 +407,7 @@ template<int C> struct SystolicState {
 
 // 16 steps. Checked = false: no boundary cell and no end cell can occur in these steps for any lane, and every k-mer
 // the lanes load lies inside its row (see the block ranges in bandedOverlapDpSystolic), so the loads are unconditional.
-template<int C, bool Checked, int Step> __device__ __forceinline__ void systolicStep(
+template<int G, int C, bool Checked, int Step> __device__ __forceinline__ void systolicStep(
     SystolicState<C>& s, int32_t eA, int32_t eB, int32_t rowEndA, int32_t nx, int32_t ny, DpScores sc, FmaUnits fu)
 {
     uint32_t ai = 0xfffffffeu;
@@ -394,11 +421,11 @@ template<int C, bool Checked, int Step> __device__ __forceinline__ void systolic
     }
     // Even step: sub-chunk A of column i. Its vertical input is the last offset of lane-1's B at column i
     // (lane 0: its own value comes back, which only the barrier offset p = 0 reads).
-    const int32_t below = __shfl_up_sync(0xffffffffu, s.HB[C - 1], 1);
+    const int32_t below = __shfl_up_sync(0xffffffffu, s.HB[C - 1], 1, G);
     systolicSubChunk<C, Checked, Step>(s.HA, s.TA, s.limA, s.i, ai, below, s.HB[0], s.bw, sc, fu);
     // Odd step: sub-chunk B of column i. Its horizontal input is the first offset of lane+1's A at column i-1
-    // (lane 31: its own value comes back, read only by barrier / padding offsets).
-    const int32_t top = __shfl_down_sync(0xffffffffu, s.HA[0], 1);
+    // (lane G-1: its own value comes back, read only by barrier / padding offsets).
+    const int32_t top = __shfl_down_sync(0xffffffffu, s.HA[0], 1, G);
     systolicSubChunk<C, Checked, Step>(s.HB, s.TB, s.limB, s.i, ai, s.HA[C - 1], top, s.bw + C, sc, fu);
     if(Checked) {
         // End-cell bookkeeping for both sub-chunks: offsets eA + cStar (row ny) and, in column nx, all rows.
@@ -415,36 +442,39 @@ template<int C, bool Checked, int Step> __device__ __forceinline__ void systolic
     s.i++; s.ap++; s.bNext++; s.jNext++;
 }
 
-template<int C, bool Checked, int... Steps> __device__ __forceinline__ void systolicStepsInPlace(
+template<int G, int C, bool Checked, int... Steps> __device__ __forceinline__ void systolicStepsInPlace(
     SystolicState<C>& s, int32_t eA, int32_t eB, int32_t rowEndA, int32_t nx, int32_t ny, DpScores sc, FmaUnits fu,
     std::integer_sequence<int, Steps...>)
 {
-    (systolicStep<C, Checked, Steps>(s, eA, eB, rowEndA, nx, ny, sc, fu), ...);
+    (systolicStep<G, C, Checked, Steps>(s, eA, eB, rowEndA, nx, ny, sc, fu), ...);
 }
 
-template<int C, bool Checked> __device__ __forceinline__ void systolicBlock(
+template<int G, int C, bool Checked> __device__ __forceinline__ void systolicBlock(
     SystolicState<C>& s, int32_t eA, int32_t eB, int32_t rowEndA, int32_t nx, int32_t ny, DpScores sc, FmaUnits fu)
 {
-    if constexpr(C <= 2) {
+    if constexpr(C <= kDpInPlaceTraceMaxC) {
         // Fully unrolled: every step adds its trace code at its own bit position of a cleared word.
 #pragma unroll
         for(int c = 0; c < C; c++) { s.TA[c] = 0; s.TB[c] = 0; }
-        systolicStepsInPlace<C, Checked>(s, eA, eB, rowEndA, nx, ny, sc, fu, std::make_integer_sequence<int, 16>{});
+        systolicStepsInPlace<G, C, Checked>(s, eA, eB, rowEndA, nx, ny, sc, fu, std::make_integer_sequence<int, 16>{});
     } else {
         constexpr int kUnroll = (C <= 4) ? 4 : (C <= 8) ? 2 : 1;
 #pragma unroll kUnroll
-        for(int step = 0; step < 16; step++) systolicStep<C, Checked, -1>(s, eA, eB, rowEndA, nx, ny, sc, fu);
+        for(int step = 0; step < 16; step++) systolicStep<G, C, Checked, -1>(s, eA, eB, rowEndA, nx, ny, sc, fu);
     }
 }
 
-template<int C> __device__ inline void bandedOverlapDpSystolic(
-    const uint32_t* __restrict__ a, uint32_t nxU, const uint32_t* __restrict__ b, uint32_t nyU, int32_t lo, int32_t hi, DpScores sc,
-    FmaUnits fu, uint32_t* __restrict__ trace, int32_t& bestScore, int32_t& bestI, int32_t& bestJ)
+// The DP of one job on a group of G lanes (G = 32: the whole warp). All 32 lanes of the warp must call it together (the
+// shuffles and the block schedule are warp-wide); live = false marks a group without a job (nx = ny = 0, no trace), which
+// steps along without storing anything. bestScore / bestI / bestJ end up in every lane of the group.
+template<int G, int C> __device__ inline void bandedOverlapDpSystolic(
+    const uint32_t* __restrict__ a, uint32_t nxU, const uint32_t* __restrict__ b, uint32_t nyU, int32_t lo, int32_t hi, bool live,
+    DpScores sc, FmaUnits fu, uint32_t* __restrict__ trace, int32_t& bestScore, int32_t& bestI, int32_t& bestJ)
 {
-    const int32_t lane = int32_t(threadIdx.x & 31u);
+    const int32_t lane = int32_t(threadIdx.x & unsigned(G - 1));
     const int32_t nx = int32_t(nxU), ny = int32_t(nyU);
     const int32_t W = hi - lo + 1;
-    const uint32_t WpadJob = dpPaddedWidth(lo, hi);
+    const uint32_t WpadJob = dpBandShape(lo, hi).wpad;
     SystolicState<C> s;
     const int32_t pA = (2 * lane) * C, pB = (2 * lane + 1) * C;         // physical offsets of the lane's sub-chunks
     const int32_t eA = pA - 1, eB = pB - 1;                             // ... as band offsets
@@ -469,34 +499,44 @@ template<int C> __device__ inline void bandedOverlapDpSystolic(
     s.bNext = b + int64_t(s.jNext);
     const int32_t rowEndA = ny + hi - eA;                   // the column in which offset eA reaches the last row
     // Steps run in blocks of 16 (one trace word per offset and block); the last block may run past the step in which
-    // lane 31 reaches column iLast: the cells beyond it feed nothing and their trace codes are never read.
-    const int32_t blocks = (iLast - iFirst + 47) >> 4;
-    // Boundary cells only occur in columns <= max(0, hi), which lane 31 leaves after step max(0, hi) - iFirst + 31.
-    // End cells (row ny, column nx) first occur in step min(nx - iFirst, ny + hi - iFirst - 64C + 32): lane 0 reaching
-    // column nx, or lane 31's last offset reaching row ny. The blocks in between run without either test, and in them
+    // lane G-1 reaches column iLast: the cells beyond it feed nothing and their trace codes are never read.
+    const int32_t blocks = live ? (iLast - iFirst + G + 15) >> 4 : 0;
+    // Boundary cells only occur in columns <= max(0, hi), which lane G-1 leaves after step max(0, hi) - iFirst + G-1.
+    // End cells (row ny, column nx) first occur in step min(nx - iFirst, ny + hi - iFirst - 2GC + G): lane 0 reaching
+    // column nx, or lane G-1's last offset reaching row ny. The blocks in between run without either test, and in them
     // every lane's column satisfies max(0, hi) < i < nx and every window row (including the element prefetched for the
     // next step) satisfies 1 <= j <= ny, so their loads need no range test: lane 0's barrier offset p = 0 sits on row
-    // i - hi - 1 >= 1 because lane 0 is 31 columns ahead of lane 31, and lane 31's prefetch index 64C - 2 + i - hi is at
-    // most ny - 1 up to step ny + hi - iFirst - 64C + 32.
-    const int32_t headBlocks = ((max(0, hi) - iFirst + 31) >> 4) + 1;
-    const int32_t firstEndStep = min(nx - iFirst, ny + hi - iFirst - 64 * C + 32);
-    const int32_t tailBlock = max(0, firstEndStep) >> 4;
+    // i - hi - 1 >= 1 because lane 0 is G-1 >= 7 columns ahead of lane G-1, and lane G-1's prefetch index 2GC - 2 + i - hi
+    // is at most ny - 1 up to step ny + hi - iFirst - 2GC + G.
+    // Several groups share a warp: a block runs unchecked only if it does so for every group, and a group without a job
+    // runs every block checked (its loads stay inside its empty rows: none).
+    int32_t headBlocks = live ? ((max(0, hi) - iFirst + G - 1) >> 4) + 1 : INT32_MAX;
+    const int32_t firstEndStep = min(nx - iFirst, ny + hi - iFirst - 2 * G * C + G);
+    int32_t tailBlock = max(0, firstEndStep) >> 4;
+    int32_t warpBlocks = blocks;
+    if constexpr(G < 32) {
+        headBlocks = __reduce_max_sync(0xffffffffu, headBlocks);
+        tailBlock = __reduce_min_sync(0xffffffffu, tailBlock);
+        warpBlocks = __reduce_max_sync(0xffffffffu, blocks);
+    }
     uint32_t* row = trace;
-    for(int32_t blk = 0; blk < blocks; blk++, row += WpadJob) {
-        if(blk < headBlocks || blk >= tailBlock) systolicBlock<C, true>(s, eA, eB, rowEndA, nx, ny, sc, fu);
-        else systolicBlock<C, false>(s, eA, eB, rowEndA, nx, ny, sc, fu);
-        // Warp-uniform, coalesced trace store of the block's 16 steps.
+    for(int32_t blk = 0; blk < warpBlocks; blk++, row += WpadJob) {
+        if(blk < headBlocks || blk >= tailBlock) systolicBlock<G, C, true>(s, eA, eB, rowEndA, nx, ny, sc, fu);
+        else systolicBlock<G, C, false>(s, eA, eB, rowEndA, nx, ny, sc, fu);
+        // Group-uniform, coalesced trace store of the block's 16 steps (a group past its last block only steps along).
+        if(blk < blocks) {
 #pragma unroll
-        for(int c = 0; c < C; c++) {
-            if(uint32_t(pA + c) < WpadJob) row[pA + c] = s.TA[c];
-            if(uint32_t(pB + c) < WpadJob) row[pB + c] = s.TB[c];
+            for(int c = 0; c < C; c++) {
+                if(uint32_t(pA + c) < WpadJob) row[pA + c] = s.TA[c];
+                if(uint32_t(pB + c) < WpadJob) row[pB + c] = s.TB[c];
+            }
         }
     }
     bestScore = s.bestScore; bestI = s.bestI; bestJ = s.bestJ;
     if(bestI != kEndCellNone) bestJ -= hi;          // bestJ was tracked as j + hi
-    // Warp reduction of the end cell.
+    // Group reduction of the end cell.
 #pragma unroll
-    for(int d = 16; d > 0; d >>= 1) {
+    for(int d = G / 2; d > 0; d >>= 1) {
         const int32_t s2 = __shfl_xor_sync(0xffffffffu, bestScore, d);
         const int32_t i2 = __shfl_xor_sync(0xffffffffu, bestI, d);
         const int32_t j2 = __shfl_xor_sync(0xffffffffu, bestJ, d);
@@ -517,7 +557,7 @@ __device__ inline uint32_t tracebackCollect(const uint32_t* __restrict__ trace, 
                                             int32_t bestI, int32_t bestJ, uint2* __restrict__ steps, int32_t pairWidth, int32_t iFirst)
 {
     const int32_t lane = int32_t(threadIdx.x & 31u);
-    const int32_t Wpad = int32_t(dpPaddedWidth(lo, hi));
+    const int32_t Wpad = int32_t(dpBandShape(lo, hi).wpad);
     int32_t i = bestI, j = bestJ;
     uint32_t n = 0;
     if(i <= 0 || j <= 0) return 0;
@@ -598,68 +638,100 @@ struct Method3Args {
     uint32_t wMax;                  // widest padded band of this launch's class (sizes the scan kernel's shared memory)
 };
 
-template<int C> __global__ void __launch_bounds__(kDpMaxWarpsPerBlock * 32)
+// The job of this lane's group in a kernel that runs 32/G jobs per warp (slots in launch order). A group without a
+// runnable job gets an empty one (live = false). Returns false when the whole warp has nothing to run.
+template<int G> __device__ __forceinline__ bool dpGroupJob(const uint32_t* __restrict__ order, uint32_t n, const DpJob* __restrict__ jobs,
+                                                           uint32_t& warpSlot, uint32_t& p, DpJob& job, bool& live)
+{
+    warpSlot = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * (32u / G);
+    if(warpSlot >= n) return false;
+    const uint32_t slot = warpSlot + (threadIdx.x & 31u) / G;
+    live = false;
+    p = 0;
+    if(slot < n) {
+        p = order[slot];
+        job = jobs[p];
+        live = job.state == kStateRun;
+    }
+    if(!live) { job = DpJob{}; job.state = kStateEmpty; }
+    return __any_sync(0xffffffffu, live);
+}
+
+// Resident blocks per SM the register allocation of the wavefront kernels aims for (the narrow classes are issue-bound and
+// want the warps).
+constexpr int dpMinBlocks(int C) { return C <= 2 ? 6 : C == 3 ? 5 : C == 4 ? 4 : C <= 8 ? 2 : 1; }
+
+template<int G, int C> __global__ void __launch_bounds__(kDpMaxWarpsPerBlock * 32, dpMinBlocks(C))
 method3Stage1Kernel(Method3Args g, DpJob* __restrict__ jobs1, uint32_t* __restrict__ trace, DpJob* __restrict__ jobs2,
                     uint2* __restrict__ ordinals)
 {
     extern __shared__ int32_t smem[];
     const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
-    const uint32_t slot = blockIdx.x * (blockDim.x >> 5) + warp;
-    if(slot >= g.n) return;
-    const uint32_t p = g.order[slot];
-    DpJob job = jobs1[p];
-    if(job.state != kStateRun) return;
-    const uint32_t* a = g.dsKmer + job.aOffset;
-    const uint32_t* b = g.dsKmer + job.bOffset;
+    uint32_t warpSlot, p;
+    DpJob job;
+    bool live;
+    if(!dpGroupJob<G>(g.order, g.n, jobs1, warpSlot, p, job, live)) return;
     int32_t bestScore, bestI, bestJ;
     if constexpr(C > 0) {
-        bandedOverlapDpSystolic<C>(a, job.nx, b, job.ny, job.lo, job.hi, g.scores, g.fma, trace + job.traceOffset, bestScore, bestI, bestJ);
+        bandedOverlapDpSystolic<G, C>(g.dsKmer + job.aOffset, job.nx, g.dsKmer + job.bOffset, job.ny, job.lo, job.hi, live, g.scores,
+                                      g.fma, live ? trace + job.traceOffset : nullptr, bestScore, bestI, bestJ);
         (void)warp;
     } else {
+        static_assert(C > 0 || G == 32, "the scan kernel runs one job per warp");
         const uint32_t stride = g.wMax + 1;
         int32_t* hPrev = smem + warp * 3 * stride;
         int32_t* hCur = hPrev + stride;
         uint32_t* traceAcc = reinterpret_cast<uint32_t*>(hCur + stride);
-        bandedOverlapDp(a, job.nx, b, job.ny, job.lo, job.hi, g.scores, hPrev, hCur, traceAcc, trace + job.traceOffset,
-                        bestScore, bestI, bestJ);
+        bandedOverlapDp(g.dsKmer + job.aOffset, job.nx, g.dsKmer + job.bOffset, job.ny, job.lo, job.hi, g.scores, hPrev, hCur, traceAcc,
+                        trace + job.traceOffset, bestScore, bestI, bestJ);
     }
     __syncwarp();
     __threadfence_block();
-    const uint32_t* oa = g.dsOrdinal + job.aOffset;
-    const uint32_t* ob = g.dsOrdinal + job.bOffset;
-    // The stage-2 ordinal slots of this candidate (min(nx,ny) >= min(n0ds,n1ds)) double as scratch for the path.
-    uint2* scratch = ordinals + jobs2[p].outOffset;
-    const uint32_t steps = tracebackCollect(trace + job.traceOffset, job.lo, job.hi, bestI, bestJ, scratch, 2 * C, C > 0 ? dpFirstColumn(job.lo) : 0);
-    int32_t offsetMin = INT32_MAX, offsetMax = INT32_MIN;
-    for(uint32_t k = lane; k < steps; k += 32) {
-        const uint2 s = scratch[k];
-        if(a[s.x] == b[s.y]) {
-            const int32_t off = int32_t(oa[s.x]) - int32_t(ob[s.y]);
-            offsetMin = min(offsetMin, off);
-            offsetMax = max(offsetMax, off);
-        }
-    }
-#pragma unroll
-    for(int d = 16; d > 0; d >>= 1) {
-        offsetMin = min(offsetMin, __shfl_xor_sync(0xffffffffu, offsetMin, d));
-        offsetMax = max(offsetMax, __shfl_xor_sync(0xffffffffu, offsetMax, d));
-    }
-    if(lane == 0) {
-        DpJob j2 = jobs2[p];
-        if(steps == 0) j2.state = kStateEmpty;                                  // :185-191
-        else {
-            // 32-bit wrap-around like the compiled reference (:222-239)
-            const int32_t bandMin = int32_t(uint32_t(offsetMin) - uint32_t(g.bandExtend));
-            const int32_t bandMax = int32_t(uint32_t(offsetMax) + uint32_t(g.bandExtend));
-            if(int32_t(uint32_t(bandMax) - uint32_t(bandMin)) > g.maxBand) j2.state = kStateEmpty;
-            else if(bandMin > bandMax || bandMax < -int32_t(j2.ny) || bandMin > int32_t(j2.nx)) j2.state = kStateSkipped;  // SeqAn MinValue -> throw
-            else {
-                j2.lo = max(bandMin, -int32_t(j2.ny));
-                j2.hi = min(bandMax, int32_t(j2.nx));
-                j2.state = kStateRun;
+    // The traceback is warp-cooperative: the warp walks the paths of its groups' jobs one after the other.
+    for(uint32_t q = 0; q < 32u / G && warpSlot + q < g.n; q++) {
+        const int32_t endI = __shfl_sync(0xffffffffu, bestI, int(q * G)), endJ = __shfl_sync(0xffffffffu, bestJ, int(q * G));
+        const uint32_t pq = __shfl_sync(0xffffffffu, p, int(q * G));
+        const DpJob jq = jobs1[pq];
+        if(jq.state != kStateRun) continue;
+        const uint32_t* a = g.dsKmer + jq.aOffset;
+        const uint32_t* b = g.dsKmer + jq.bOffset;
+        const uint32_t* oa = g.dsOrdinal + jq.aOffset;
+        const uint32_t* ob = g.dsOrdinal + jq.bOffset;
+        // The stage-2 ordinal slots of this candidate (min(nx,ny) >= min(n0ds,n1ds)) double as scratch for the path.
+        uint2* scratch = ordinals + jobs2[pq].outOffset;
+        const uint32_t steps = tracebackCollect(trace + jq.traceOffset, jq.lo, jq.hi, endI, endJ, scratch, 2 * C, C > 0 ? dpFirstColumn(jq.lo) : 0);
+        int32_t offsetMin = INT32_MAX, offsetMax = INT32_MIN;
+        for(uint32_t k = lane; k < steps; k += 32) {
+            const uint2 s = scratch[k];
+            if(a[s.x] == b[s.y]) {
+                const int32_t off = int32_t(oa[s.x]) - int32_t(ob[s.y]);
+                offsetMin = min(offsetMin, off);
+                offsetMax = max(offsetMax, off);
             }
         }
-        jobs2[p] = j2;
+#pragma unroll
+        for(int d = 16; d > 0; d >>= 1) {
+            offsetMin = min(offsetMin, __shfl_xor_sync(0xffffffffu, offsetMin, d));
+            offsetMax = max(offsetMax, __shfl_xor_sync(0xffffffffu, offsetMax, d));
+        }
+        if(lane == 0) {
+            DpJob j2 = jobs2[pq];
+            if(steps == 0) j2.state = kStateEmpty;                                  // :185-191
+            else {
+                // 32-bit wrap-around like the compiled reference (:222-239)
+                const int32_t bandMin = int32_t(uint32_t(offsetMin) - uint32_t(g.bandExtend));
+                const int32_t bandMax = int32_t(uint32_t(offsetMax) + uint32_t(g.bandExtend));
+                if(int32_t(uint32_t(bandMax) - uint32_t(bandMin)) > g.maxBand) j2.state = kStateEmpty;
+                else if(bandMin > bandMax || bandMax < -int32_t(j2.ny) || bandMin > int32_t(j2.nx)) j2.state = kStateSkipped;  // SeqAn MinValue -> throw
+                else {
+                    j2.lo = max(bandMin, -int32_t(j2.ny));
+                    j2.hi = min(bandMax, int32_t(j2.nx));
+                    j2.state = kStateRun;
+                }
+            }
+            jobs2[pq] = j2;
+        }
+        __syncwarp();
     }
 }
 
@@ -667,10 +739,11 @@ method3Stage1Kernel(Method3Args g, DpJob* __restrict__ jobs1, uint32_t* __restri
 // largest ordinal offset over the matching diagonal steps of the optimal path (src/AssemblerAlign3.cpp:193-239), so
 // every cell carries that pair along with its score and inherits it from the predecessor the recurrence picks: the
 // same information a traceback from that cell would collect, with no trace to write or walk.
-// Layout: lane l owns the R consecutive rows j = R*l + 1 .. R*l + R of b (its k-mers and ordinals stay in registers),
-// and in step t works on column i = t - l + 1; the only inter-lane traffic is lane l-1's last row (score and pair) of
-// the same column, one step earlier. Rows beyond ny and columns outside 1..nx are dead: nothing live reads them.
-// Covers ny <= 32*R (R <= 16); longer downsampled reads take method3Stage1Kernel. Same recurrence, tie-break and
+// Layout: a job runs on a group of G lanes (G = 8, 16 or 32; 32/G jobs per warp). Lane l of the group owns the R
+// consecutive rows j = R*l + 1 .. R*l + R of b (its k-mers and ordinals stay in registers), and in step t works on column
+// i = t - l + 1; the only inter-lane traffic is lane l-1's last row (score and pair) of the same column, one step
+// earlier. Rows beyond ny and columns outside 1..nx are dead: nothing live reads them.
+// Covers ny <= G*R (R <= 16); longer downsampled reads take method3Stage1Kernel. Same recurrence, tie-break and
 // end-cell rules as bandedOverlapDp.
 // The (smallest, largest) matching ordinal offset of a path travels as ONE packed value: low half = the smallest offset,
 // high half = MINUS the largest, both as signed 16-bit numbers, so that one packed minimum (VIMNMX.S16x2) updates both and
@@ -692,15 +765,14 @@ __device__ __forceinline__ uint32_t packOffsetPair(int32_t lowHalf, int32_t high
     return (uint32_t(lowHalf) & 0xffffu) | (uint32_t(highHalf) << 16);
 }
 
-template<int R> __global__ void __launch_bounds__(kDpMaxWarpsPerBlock * 32)
+template<int G, int R> __global__ void __launch_bounds__(kDpMaxWarpsPerBlock * 32)
 method3Stage1ForwardKernel(Method3Args g, const DpJob* __restrict__ jobs1, DpJob* __restrict__ jobs2)
 {
-    const int32_t lane = int32_t(threadIdx.x & 31u);
-    const uint32_t slot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    if(slot >= g.n) return;
-    const uint32_t p = g.order[slot];
-    const DpJob job = jobs1[p];
-    if(job.state != kStateRun) return;
+    const int32_t lane = int32_t(threadIdx.x & unsigned(G - 1));
+    uint32_t warpSlot, p;
+    DpJob job;
+    bool live;
+    if(!dpGroupJob<G>(g.order, g.n, jobs1, warpSlot, p, job, live)) return;
     const uint32_t* __restrict__ a = g.dsKmer + job.aOffset;
     const uint32_t* __restrict__ oa = g.dsOrdinal + job.aOffset;
     const int32_t nx = int32_t(job.nx), ny = int32_t(job.ny);
@@ -721,18 +793,19 @@ method3Stage1ForwardKernel(Method3Args g, const DpJob* __restrict__ jobs1, DpJob
         }
         H[r] = 0; P[r] = kPairNoDiagonalStep;
     }
-    const int32_t lastLane = (ny - 1) / R, rLast = (ny - 1) % R;        // where row ny lives
+    const int32_t lastLane = live ? (ny - 1) / R : 0, rLast = live ? (ny - 1) % R : -1;        // where row ny lives
     int32_t upH = 0;                                                    // row R*lane of the previous column
     uint32_t upP = kPairNoDiagonalStep;
     int32_t bestScore = 0, bestI = kEndCellNone, bestJ = kEndCellNone;
     uint32_t bestP = kPairNoDiagonalStep;
 
-    const int32_t steps = nx + lastLane;                                // lanes beyond lastLane only hold dead rows
+    int32_t steps = nx + lastLane;                                      // lanes beyond lastLane only hold dead rows
+    if constexpr(G < 32) steps = __reduce_max_sync(0xffffffffu, steps);  // a group past its last step only steps along
 #pragma unroll 2
     for(int32_t t = 0; t < steps; t++) {
         // Row R*lane of the current column: lane-1's last row, computed one step ago (row 0 for lane 0).
-        int32_t inH = __shfl_up_sync(0xffffffffu, H[R - 1], 1);
-        uint32_t inP = __shfl_up_sync(0xffffffffu, P[R - 1], 1);
+        int32_t inH = __shfl_up_sync(0xffffffffu, H[R - 1], 1, G);
+        uint32_t inP = __shfl_up_sync(0xffffffffu, P[R - 1], 1, G);
         if(lane == 0) { inH = 0; inP = kPairNoDiagonalStep; }
         const int32_t i = t - lane + 1;
         if(uint32_t(i - 1) < uint32_t(nx)) {
@@ -761,7 +834,7 @@ method3Stage1ForwardKernel(Method3Args g, const DpJob* __restrict__ jobs1, DpJob
             // cells score 0 and come first, so only positive scores can win under the first-maximum rule).
             if(lane == lastLane) {
                 int32_t h = 0; uint32_t pr = 0;
-                switch(rLast) {                  // warp-uniform; a jump instead of R selects per value
+                switch(rLast) {                  // group-uniform; a jump instead of R selects per value
 #define SHB_PICK_ROW(k) case k: if constexpr(k < R) { h = H[k]; pr = P[k]; } break;
                 SHB_PICK_ROW(0) SHB_PICK_ROW(1) SHB_PICK_ROW(2) SHB_PICK_ROW(3) SHB_PICK_ROW(4) SHB_PICK_ROW(5) SHB_PICK_ROW(6) SHB_PICK_ROW(7)
                 SHB_PICK_ROW(8) SHB_PICK_ROW(9) SHB_PICK_ROW(10) SHB_PICK_ROW(11) SHB_PICK_ROW(12) SHB_PICK_ROW(13) SHB_PICK_ROW(14) SHB_PICK_ROW(15)
@@ -780,9 +853,9 @@ method3Stage1ForwardKernel(Method3Args g, const DpJob* __restrict__ jobs1, DpJob
         }
         upH = inH; upP = inP;
     }
-    // Maximum score, then the visiting order of the end-cell rule.
+    // Maximum score, then the visiting order of the end-cell rule (over the lanes of the group).
 #pragma unroll
-    for(int d = 16; d > 0; d >>= 1) {
+    for(int d = G / 2; d > 0; d >>= 1) {
         const int32_t s2 = __shfl_xor_sync(0xffffffffu, bestScore, d);
         const int32_t i2 = __shfl_xor_sync(0xffffffffu, bestI, d);
         const int32_t j2 = __shfl_xor_sync(0xffffffffu, bestJ, d);
@@ -791,7 +864,7 @@ method3Stage1ForwardKernel(Method3Args g, const DpJob* __restrict__ jobs1, DpJob
             bestScore = s2; bestI = i2; bestJ = j2; bestP = p2;
         }
     }
-    if(lane == 0) {
+    if(lane == 0 && live) {
         DpJob j2 = jobs2[p];
         const uint32_t lowHalf = bestP & 0xffffu;
         if(bestI == kEndCellNone || lowHalf == (kPairNoDiagonalStep & 0xffffu)) j2.state = kStateEmpty;        // :185-191
@@ -815,7 +888,7 @@ method3Stage1ForwardKernel(Method3Args g, const DpJob* __restrict__ jobs1, DpJob
 }
 
 // Stage 2 / generic banded alignment on full marker rows, in three launches:
-//   bandedAlignKernel<C>   one warp per job: the DP; writes the trace and the end cell;
+//   bandedAlignKernel<G,C> one group of G lanes per job: the DP; writes the trace and the end cell;
 //   tracebackKernel        one THREAD per job: walks the trace (a serial, latency-bound pointer chase that a warp could
 //                          only execute redundantly on its 32 lanes) and writes every diagonal step, last step first;
 //   filterStepsKernel      one warp per job: keeps the steps on equal k-mers; counts[p] receives how many.
@@ -828,26 +901,24 @@ struct BandedArgs {
     uint32_t wMax;                  // widest padded band of this launch's class (sizes the scan kernel's shared memory)
 };
 
-// Resident blocks per SM the register allocation aims for (the narrow classes are issue-bound and want the warps).
-constexpr int dpMinBlocks(int C) { return C == 1 ? 7 : C == 2 ? 6 : C == 3 ? 5 : C == 4 ? 4 : C <= 8 ? 2 : 1; }
-
-template<int C> __global__ void __launch_bounds__(kDpMaxWarpsPerBlock * 32, dpMinBlocks(C))
+template<int G, int C> __global__ void __launch_bounds__(kDpMaxWarpsPerBlock * 32, dpMinBlocks(C))
 bandedAlignKernel(BandedArgs g, const DpJob* __restrict__ jobs, uint32_t* __restrict__ trace, int2* __restrict__ endCells)
 {
     extern __shared__ int32_t smem[];
-    const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & 31u;
-    const uint32_t slot = blockIdx.x * (blockDim.x >> 5) + warp;
-    if(slot >= g.n) return;
-    const uint32_t p = g.order[slot];
-    const DpJob job = jobs[p];
-    if(job.state != kStateRun) return;
+    const unsigned warp = threadIdx.x >> 5, lane = threadIdx.x & unsigned(G - 1);
+    uint32_t warpSlot, p;
+    DpJob job;
+    bool live;
+    if(!dpGroupJob<G>(g.order, g.n, jobs, warpSlot, p, job, live)) return;
     const uint32_t* a = g.kmerIds + job.aOffset;
     const uint32_t* b = g.kmerIds + job.bOffset;
     int32_t bestScore, bestI, bestJ;
     if constexpr(C > 0) {
-        bandedOverlapDpSystolic<C>(a, job.nx, b, job.ny, job.lo, job.hi, g.scores, g.fma, trace + job.traceOffset, bestScore, bestI, bestJ);
+        bandedOverlapDpSystolic<G, C>(a, job.nx, b, job.ny, job.lo, job.hi, live, g.scores, g.fma, live ? trace + job.traceOffset : nullptr,
+                                      bestScore, bestI, bestJ);
         (void)warp;
     } else {
+        static_assert(C > 0 || G == 32, "the scan kernel runs one job per warp");
         const uint32_t stride = g.wMax + 1;
         int32_t* hPrev = smem + warp * 3 * stride;
         int32_t* hCur = hPrev + stride;
@@ -855,13 +926,7 @@ bandedAlignKernel(BandedArgs g, const DpJob* __restrict__ jobs, uint32_t* __rest
         bandedOverlapDp(a, job.nx, b, job.ny, job.lo, job.hi, g.scores, hPrev, hCur, traceAcc, trace + job.traceOffset,
                         bestScore, bestI, bestJ);
     }
-    if(lane == 0) endCells[p] = make_int2(bestI, bestJ);
-}
-
-// Offsets per sub-chunk of the wavefront kernel that handles a padded band width (0: the scan kernel, by-column trace).
-__host__ __device__ inline uint32_t dpWavefrontC(uint32_t Wpad)
-{
-    return Wpad <= 256 ? Wpad / 64 : Wpad <= 384 ? 6 : Wpad <= 512 ? 8 : Wpad <= 768 ? 12 : Wpad <= kDpWavefrontMaxWidth ? 16 : 0;
+    if(lane == 0 && live) endCells[p] = make_int2(bestI, bestJ);
 }
 
 // A run of consecutive diagonal steps (x0 - k, y0 - k), k = 0 .. length-1, as the traceback emits it (last step first):
@@ -882,8 +947,8 @@ tracebackKernel(uint32_t n, const uint32_t* __restrict__ order, const DpJob* __r
     int32_t i = end.x, j = end.y;
     uint32_t count = 0;
     if(job.state == kStateRun && i > 0 && j > 0) {
-        const uint32_t Wpad = dpPaddedWidth(job.lo, job.hi);
-        const uint32_t C = dpWavefrontC(Wpad);
+        const DpShape shape = dpBandShape(job.lo, job.hi);
+        const uint32_t Wpad = shape.wpad, C = shape.c;
         // By-step layout: the code of cell (i, p) sits in step t = (i - iFirst) + p / (2C); by-column layout: t = i.
         const int32_t iFirst = C ? dpFirstColumn(job.lo) : 0;
         const uint32_t reciprocal = C ? (65536u + 2u * C - 1u) / (2u * C) : 0u;      // p / (2C) == (p * reciprocal) >> 16 for p < 1024
@@ -1208,7 +1273,7 @@ static __global__ void method3SetupKernel(const uint32_t* __restrict__ candidate
         j2.bOffset = toc[o1]; j2.ny = uint32_t(toc[o1 + 1] - toc[o1]);
         j2.lo = -int32_t(j2.ny); j2.hi = int32_t(j2.nx); j2.traceOffset = 0; j2.outOffset = 0; j2.pad = 0;
         j2.state = (j2.nx == 0 || j2.ny == 0) ? kStateEmpty : kStateRun;
-        if(j2.state == kStateRun && dpPaddedWidth(j2.lo, j2.hi) > maxWidth) { j2.state = kStateSkipped; atomicAdd(tooWide, 1ull); }
+        if(j2.state == kStateRun && dpBandShape(j2.lo, j2.hi).wpad > maxWidth) { j2.state = kStateSkipped; atomicAdd(tooWide, 1ull); }
         jobs2[p] = j2;
         outCount[p] = min(j2.nx, j2.ny);
         return;
@@ -1225,7 +1290,7 @@ static __global__ void method3SetupKernel(const uint32_t* __restrict__ candidate
     // ordinal offset does not fit the kernel's 16-bit offset pair. pad = 1 marks the forward-kernel jobs for the class sort.
     const bool forward = j1.ny <= kStage1ForwardMaxRows && max(j2.nx, j2.ny) <= kStage1ForwardMaxMarkers;
     j1.pad = forward ? 1u : 0u;
-    if(j1.state == kStateRun && !forward && dpPaddedWidth(j1.lo, j1.hi) > maxWidth) {
+    if(j1.state == kStateRun && !forward && dpBandShape(j1.lo, j1.hi).wpad > maxWidth) {
         j1.state = kStateSkipped; atomicAdd(tooWide, 1ull);
     }
     j2.state = (j1.state == kStateEmpty) ? kStateEmpty : kStateSkipped;     // stage 1 overwrites it when it runs
@@ -1244,32 +1309,48 @@ static __global__ void setTraceOffsetsKernel(DpJob* __restrict__ jobs, uint32_t 
     if(outOffsets) jobs[p].outOffset = outOffsets[p];
 }
 
-constexpr int kDpLengthKeyBits = 11, kDpClassKeyBits = 5;
-constexpr uint32_t kDpLengthKeyMax = (1u << kDpLengthKeyBits) - 1u, kDpClassNone = (1u << kDpClassKeyBits) - 1u;
+// Classes of the forward kernel (method 3, stage 1 without a trace): groups of `lanes` lanes with `rows` rows per lane
+// hold ny <= lanes * rows downsampled markers: steps of 8 rows up to 128 on groups of 8 lanes, of 16 up to 256 on groups
+// of 16, then 384 and 512 on whole warps.
+struct DpForwardClass { uint32_t lanes, rows; };
+constexpr uint32_t kDpForwardClassCount = 26;
+__host__ __device__ constexpr DpForwardClass dpForwardClassAt(uint32_t k)
+{
+    return k < 16 ? DpForwardClass{8u, k + 1u} : k < 24 ? DpForwardClass{16u, k - 7u} : DpForwardClass{32u, k == 24 ? 12u : 16u};
+}
+static_assert(dpForwardClassAt(kDpForwardClassCount - 1).lanes * dpForwardClassAt(kDpForwardClassCount - 1).rows == kStage1ForwardMaxRows,
+              "the forward classes cover every row count the forward kernel takes");
 
-// Sort key of a DP job: band class, then longest sequence first (load balance inside a launch).
-// classLimits[k] = widest padded band of class k; jobs that do not run get class kDpClassNone.
-// forwardClasses > 0 (method 3, stage 1): jobs of at most classLimits[forwardClasses-1] rows go to the forward kernel,
-// class k = first k with ny <= classLimits[k]; the others keep their band class, shifted up by forwardClasses.
-static __global__ void dpClassKeysKernel(const DpJob* __restrict__ jobs, uint32_t n, const uint32_t* __restrict__ classLimits,
-                                         uint32_t classCount, uint32_t forwardClasses, uint64_t* __restrict__ keys, uint32_t* __restrict__ vals)
+constexpr int kDpLengthKeyBits = 10, kDpClassKeyBits = 6;
+constexpr uint32_t kDpLengthKeyMax = (1u << kDpLengthKeyBits) - 1u, kDpClassNone = (1u << kDpClassKeyBits) - 1u;
+static_assert(kDpForwardClassCount + kDpClassCount < kDpClassNone, "class key too narrow");
+
+// Sort key of a DP job: class, then longest first (load balance inside a launch; the jobs that share a warp differ by
+// less than one 16-step block). Band class: dpBandShape; jobs that do not run get class kDpClassNone.
+// forward (method 3, stage 1): the jobs marked for the forward kernel take its classes (dpForwardClassAt), the others
+// their band class, shifted up by kDpForwardClassCount.
+static __global__ void dpClassKeysKernel(const DpJob* __restrict__ jobs, uint32_t n, bool forward, uint64_t* __restrict__ keys,
+                                         uint32_t* __restrict__ vals)
 {
     const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
     if(p >= n) return;
     const DpJob j = jobs[p];
-    uint32_t cls = 255;
+    uint32_t cls = kDpClassNone;
     if(j.state == kStateRun) {
-        if(forwardClasses && j.pad) {           // marked by method3SetupKernel: few enough rows and short enough reads
-            for(uint32_t k = 0; k < forwardClasses; k++) if(j.ny <= classLimits[k]) { cls = k; break; }
+        if(forward && j.pad) {                  // marked by method3SetupKernel: few enough rows and short enough reads
+            for(uint32_t k = 0; k < kDpForwardClassCount; k++) {
+                const DpForwardClass f = dpForwardClassAt(k);
+                if(j.ny <= f.lanes * f.rows) { cls = k; break; }
+            }
         } else {
-            const uint32_t Wpad = dpPaddedWidth(j.lo, j.hi);
-            for(uint32_t k = 0; k < classCount; k++) if(Wpad <= classLimits[k]) { cls = forwardClasses + k; break; }
+            const DpShape s = dpBandShape(j.lo, j.hi);
+            if(s.wpad <= dpClassAt(s.cls).wMax) cls = (forward ? kDpForwardClassCount : 0u) + s.cls;
         }
     }
     // 16-bit key (two radix passes): class, then the number of columns the kernel visits in units of 16, longest first.
     const int32_t active = dpLastColumn(j.nx, j.ny, j.hi) - dpFirstColumn(j.lo);
     const uint32_t length = min(uint32_t(active > 0 ? active : 0) >> 4, kDpLengthKeyMax);
-    keys[p] = (uint64_t(min(cls, kDpClassNone)) << kDpLengthKeyBits) | uint64_t(kDpLengthKeyMax - length);
+    keys[p] = (uint64_t(cls) << kDpLengthKeyBits) | uint64_t(kDpLengthKeyMax - length);
     vals[p] = p;
 }
 
