@@ -21,6 +21,7 @@ struct LowHashState {
     shb_lowhash_params p{};
     uint64_t log2BucketCount = 0, bucketMask = 0, hashThreshold = 0, capacity = 0;
     uint32_t readBits = 1, slabGroup = 0;
+    uint32_t queueCapacityOverride = 0; // SHB_LOWHASH_QUEUE_CAPACITY (test hook), 0 = derived from hashFraction
     bool aggregateByRead = false;       // pair hits are counted per read in shared memory before they reach the accumulator
     LowHashAccumulator acc;
     uint64_t lowHashCount = 0, pairCount = 0, sweepLaunches = 0;

@@ -233,6 +233,12 @@ void lowhashBegin(shb_context* c, const shb_lowhash_params& p)
         const long long v = std::atoll(e);
         if(v > 0) S.acc.rawLimit = uint64_t(v);
     }
+    // Test hook: the sweep's shared-memory queue holds this many low hashes per tile instead of the number derived from
+    // hashFraction (lowhashSweep), clamped to 1 ... kSweepQueueMax; the hits beyond it take the sweep's inline path.
+    if(const char* e = std::getenv("SHB_LOWHASH_QUEUE_CAPACITY")) {
+        const long long v = std::atoll(e);
+        if(v > 0) S.queueCapacityOverride = uint32_t(std::min<long long>(v, kSweepQueueMax));
+    }
     g_launchCount = 0;
     const uint64_t R = c->readCountTotal;
 
@@ -293,6 +299,7 @@ void lowhashSweep(shb_context* c, uint64_t iterationBegin, uint32_t group, unsig
         {
             const double expected = double(kSweepTile) * double(group) * S.p.hashFraction;
             a.queueCapacity = uint32_t(std::min<double>(kSweepQueueMax, std::max<double>(kSweepQueueMin, 1.5 * expected + 64.)));
+            if(S.queueCapacityOverride) a.queueCapacity = S.queueCapacityOverride;
         }
         const uint32_t tileCount = uint32_t(ceilDiv(M, kSweepTile));
         if(tileCount && (c->sweepTileGeneration != c->markerGeneration || c->sweepTileFirstRead.capacity() < tileCount)) {

@@ -106,16 +106,34 @@ def test_tinytest_pin_through_host_call(ctx, golden_dir):
     assert res.log2BucketCount == 16
 
 
-@pytest.mark.parametrize("m", [1, 2, 3, 6, 7, 8, 9, 12])
+@pytest.mark.parametrize("m", [1, 2, 3, 6, 7, 8, 9, 12, 13, 16, 31, 32])
 def test_feature_lengths_against_oracle(ctx, m):
     from shasta_b200 import capi
+    import test_gpu_lowhash_paths as P
     d = synth.generate(synth.SynthParams(reads=120, k=10, genome_markers=15000, n50_bases=12000, min_bases=6000, seed=40 + m))
     kw = dict(m=m, hashFraction=0.02, minHashIterationCount=5, minBucketSize=0, maxBucketSize=20, minFrequency=1)
+    if m > 8:
+        # Generic kernel (m > 8): some low hash of the launch starts at the last position of a full tile, so that its
+        # feature reads m - 1 words of the halo that follows the tile (at m = 32, up to its last word).
+        M = int(d["toc"][-1])
+        local = np.arange(P.TILE - m + 1, P.TILE)
+        positions = (np.arange(1, M // P.TILE)[:, None] * P.TILE + local[None, :] - P.TILE).ravel()
+        h = P.feature_hashes(d["kmer"], m, [37 * s for s in range(5)], positions=positions)
+        halo = (h < np.uint64(P.hash_threshold(0.02))).any(0)
+        assert (positions[halo] % P.TILE == P.TILE - 1).any()
     ctx.set_markers(d["toc"], d["data"], d["flags"])
     cand, stats, _, _ = ctx.lowhash0(capi.make_lowhash_params(**kw))
     oc, os_, _ = B.oracle_lowhash0(d["toc"], d["data"], d["flags"], B.LowHashParams(**kw))
     assert np.array_equal(cand, oc)
     assert np.array_equal(stats, os_)
+
+
+def test_feature_length_33_is_refused(ctx):
+    from shasta_b200 import capi
+    d = synth.generate(synth.SynthParams(reads=20, k=10, genome_markers=6000, n50_bases=9000, min_bases=4000, seed=3))
+    ctx.set_markers(d["toc"], d["data"], d["flags"])
+    with pytest.raises(capi.ShastaB200Error, match="MinHash.m must be between 1 and 32"):
+        ctx.lowhash0(capi.make_lowhash_params(m=33))
 
 
 def test_edge_cases_against_oracle(ctx):
