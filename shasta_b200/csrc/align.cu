@@ -261,7 +261,7 @@ void buildDownsampled(shb_context* c, uint32_t k, double factor)
     // src/AssemblerAlign3.cpp:71-72
     const uint32_t hashThreshold = uint32_t(factor * double(std::numeric_limits<uint32_t>::max()));
     ds.dsToc.reserve(uint64_t(rows) + 1);
-    const uint32_t chunk = 1u << 27;
+    const uint32_t chunk = envCount("SHB_DOWNSAMPLE_CHUNK", 1u << 27);     // test hook: small sets cross chunk seams
     c->flagsBuf.reserve(std::min<uint64_t>(chunk, M) + 1);
     c->indexBuf.reserve(std::min<uint64_t>(chunk, M) + 1);
     c->scanWs.reserve(scanWorkspaceElements(chunk));
@@ -311,7 +311,7 @@ void buildSortedMarkers(shb_context* c, uint32_t k)
     const std::vector<uint64_t>& toc = c->tocHost;
     DeviceBuffer<uint64_t> keysA, keysB;
     DeviceBuffer<uint32_t> valsA, valsB;
-    const uint64_t chunkLimit = 1ull << 28;
+    const uint64_t chunkLimit = envCount("SHB_ALIGN4_SORT_CHUNK", 1u << 28);     // test hook: small sets make many row chunks
     uint32_t rowBegin = 0;
     while(rowBegin < rows) {
         uint32_t rowEnd = rowBegin + 1;
@@ -337,14 +337,6 @@ void buildSortedMarkers(shb_context* c, uint32_t k)
     }
     SHB_CUDA(cudaStreamSynchronize(st));
     sc.sortedGeneration = c->markerGeneration;
-}
-
-uint32_t envCount(const char* name, uint32_t dflt)
-{
-    const char* v = getenv(name);
-    if(!v) return dflt;
-    const long x = strtol(v, nullptr, 10);
-    return x > 0 ? uint32_t(x) : dflt;
 }
 
 void parallelMemcpy(uint8_t* dst, const uint8_t* src, uint64_t n)

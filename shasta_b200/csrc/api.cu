@@ -142,7 +142,8 @@ shb_status shb_set_markers(shb_context* c, uint64_t readCountTotal, uint64_t rea
         SHB_REQUIRE(markerData7 != nullptr || M == 0, SHB_ERR_INVALID, "Null marker data.");
         c->kmerIdsOwned.reserve(M + 64);
         // Stream the 7-byte records through two staging buffers; only the uint32 SoA stays resident.
-        const uint64_t chunkMarkers = 32ull << 20;                     // multiple of 1024
+        // SHB_MARKER_UPLOAD_CHUNK: test hook that shrinks the staging chunk so that small marker sets cross its seams.
+        const uint64_t chunkMarkers = (uint64_t(envCount("SHB_MARKER_UPLOAD_CHUNK", 32u << 20)) + 1023) & ~1023ull;  // multiple of 1024
         const uint64_t chunkBytes = chunkMarkers * 7;
         DeviceBuffer<uint8_t> staging[2];
         for(uint64_t begin = 0, k = 0; begin < M; begin += chunkMarkers, k++) {

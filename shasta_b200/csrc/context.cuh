@@ -4,9 +4,19 @@
 #include "common.cuh"
 #include "primitives.cuh"
 
+#include <cstdlib>
 #include <vector>
 
 namespace shb {
+// A positive count from the environment (the SHB_* test hooks that shrink batch and chunk sizes), else dflt.
+inline uint32_t envCount(const char* name, uint32_t dflt)
+{
+    const char* v = std::getenv(name);
+    if(!v) return dflt;
+    const long x = std::strtol(v, nullptr, 10);
+    return x > 0 ? uint32_t(x) : dflt;
+}
+
 constexpr int kMaxFusedIterations = 16;         // LowHash iterations hashed per pass over the k-mer ids (one slab each)
 struct LowHashAccumulator {
     uint64_t count = 0;     // reduced (pairKey, count) items in the acc ping-pong buffers

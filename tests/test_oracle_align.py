@@ -8,6 +8,7 @@ The overlap DP's tie-break rule is 'parity unpinned' (SeqAn absent, SURVEY.md F4
   * the whole Align4 front end (cells, searches, components, band, selection) against the compiled Align4.cpp,
   * DP optimality properties that hold for any correct implementation (score = brute force, path validity).
 """
+import ctypes as C
 import os
 import sys
 
@@ -52,6 +53,28 @@ def test_reference_selftest_and_compress_vectors():
     # Format 4 (|skip| >= 2^19) and a negative skip
     o = np.array([[2000000, 5], [2000001, 6], [2000010, 1000000]], np.uint32)
     assert np.array_equal(B.oracle_compress(o), recorded("align", "compress_format4", B.ref_compress, o))
+
+
+def _ref_murmurhash2_u64(n):
+    lib = B.ref_lib()
+    out = np.empty(len(n), np.uint32)
+    for i, x in enumerate(n.tolist()):
+        v = C.c_uint64(x)
+        out[i] = lib.ref_murmurhash2(C.byref(v), 8, 13477)
+    return out
+
+
+def test_downsampling_hash_at_k16():
+    # At k = 16 the sum n = kmerId + rc(kmerId) can reach 2^32, so the second word of the 8-byte MurmurHash2 is not zero
+    # (src/AssemblerKmers.cpp:182-186): the oracle's hash and the tests' numpy model against the reference's MurmurHash2 of n.
+    import test_gpu_align_limits as AL
+    ids = np.random.default_rng(16).integers(0, 1 << 32, 100000, dtype=np.uint64).astype(np.uint32)
+    n = ids.astype(np.uint64) + synth.reverse_complement_kmer(ids, 16).astype(np.uint64)
+    assert (n >> np.uint64(32) != 0).sum() > 40000
+    expected = recorded("align", "downsampling_hash_k16", _ref_murmurhash2_u64, n)
+    lib = B.oracle_lib()
+    assert np.array_equal(np.array([lib.orc_kmer_downsampling_hash(x, 16) for x in ids.tolist()], np.uint32), expected)
+    assert np.array_equal(AL.downsampling_hash(ids, 16), expected)
 
 
 def _brute_score(a, b, match, mismatch, gap, band=None):
