@@ -298,6 +298,36 @@ shb_status shb_compute_alignment_table(shb_context* ctx, const void* alignmentDa
 shb_status shb_compute_candidate_table(shb_context* ctx, const void* candidates, uint64_t candidateCount,
                                        uint64_t readCount, uint64_t** tableToc, uint64_t** tableData);
 
+// ---- flagPalindromicReads (src/AssemblerAlign.cpp:652-770) ----------------------------------------------------------
+// The arguments of Assembler::flagPalindromicReads. threadCount is accepted and ignored.
+typedef struct {
+    uint32_t maxSkip, maxDrift, maxMarkerFrequency, deltaThreshold;
+    double alignedFractionThreshold, nearDiagonalFractionThreshold;
+    uint64_t threadCount;
+} shb_palindromic_params;
+typedef struct {
+    uint64_t readCount, palindromicReadCount;
+    uint64_t exactReadCount;        // reads the prefilter could not decide: they got the alignment graph and its path
+    uint64_t vertexCount, edgeCount, heapPushCount, heapsortFallbackCount;     // over those reads
+    double totalMs, exactMs;        // wall time of the call and of its exact phase
+    uint64_t kernelLaunches;
+} shb_palindromic_result;
+// Flags the palindromic reads of the markers held by ctx (set by shb_set_markers* or shb_find_markers): bit 0 of every
+// read's flags is reset, then set where the alignment of the read against its reverse complement (alignment method 0)
+// passes both thresholds, exactly as the reference decides it. Bits 1-7 are kept. The context's flags are updated in
+// place, so a following shb_lowhash0 / shb_compute_alignments sees them. readFlags (in/out, R bytes), alignedMarkerCount
+// and nearDiagonalMarkerCount (R entries each) are optional. The counts are the reference's for the reads that got the
+// alignment (exactReadCount of them, every read the reference flags among them); for every other read they are the
+// bounds that decided it without an alignment: the number of alignment-graph vertices and of those within
+// deltaThreshold of the diagonal, saturated to 32 bits. A context that holds only a read range returns SHB_ERR_STATE.
+shb_status shb_flag_palindromic_reads(shb_context* ctx, const shb_palindromic_params* params, uint8_t* readFlags,
+                                      uint32_t* alignedMarkerCount, uint32_t* nearDiagonalMarkerCount,
+                                      shb_palindromic_result* result);
+// The alignment of one read against its reverse complement that flagPalindromicReads uses (alignOrientedReads(readId, 0,
+// readId, 1) with method 0): *ordinals = count (ordinal0, ordinal1) pairs, release with shb_free.
+shb_status shb_palindromic_read_alignment(shb_context* ctx, uint64_t readId, const shb_palindromic_params* params,
+                                          uint32_t** ordinals, uint64_t* count);
+
 /* Replaces Assembler::createReadGraph, ReadGraph.creationMethod 0 (src/AssemblerReadGraph.cpp:35-175): for each read the
  * best maxAlignmentCount alignments by (markerCount, alignmentId), both descending, are kept; an alignment kept by either
  * of its reads becomes two read graph edges (the edge and its reverse complement), in alignmentId order.

@@ -233,6 +233,27 @@ class Assembler:
         """Assembler::accessSortedMarkers (src/PythonModule.cpp:213-214): nothing to open, see computeSortedMarkers."""
         self.checkMarkersAreOpen()
 
+    def flagPalindromicReads(self, maxSkip, maxDrift, maxMarkerFrequency, alignedFractionThreshold,
+                             nearDiagonalFractionThreshold, deltaThreshold, threadCount=0):
+        """Assembler::flagPalindromicReads (src/AssemblerAlign.cpp:652-770, binding src/PythonModule.cpp:251-259) on the
+        device: bit 0 of every read's flags is reset, then set on the reads whose alignment with their own reverse
+        complement passes both thresholds. Data/ReadFlags is rewritten; the markers stay on the device, with the new flags,
+        for the LowHash0 and alignment calls that follow. threadCount is accepted and ignored."""
+        from . import capi
+        ctx = self._upload_markers()
+        toc, data, flags = self._markers
+        flags = np.array(flags, dtype=np.uint8)
+        params = capi.make_palindromic_params(maxSkip=maxSkip, maxDrift=maxDrift, maxMarkerFrequency=maxMarkerFrequency,
+                                              alignedFractionThreshold=alignedFractionThreshold,
+                                              nearDiagonalFractionThreshold=nearDiagonalFractionThreshold,
+                                              deltaThreshold=deltaThreshold, threadCount=threadCount)
+        _, _, res = capi.flag_palindromic_reads(ctx, params, read_flags=flags, want_counts=False)
+        mm_write_vector(self._name("ReadFlags"), flags, object_size=1)
+        self._markers = (toc, data, flags)
+        readCount = len(flags)
+        print(f"Flagged {res.palindromicReadCount} reads as palindromic out of {readCount} total.")
+        print(f"Palindromic fraction is {_ostream_double(res.palindromicReadCount / readCount if readCount else float('nan'))}")
+
     def alignOrientedReads4(self, readId0, strand0, readId1, strand1, deltaX, deltaY, minEntryCountPerCell,
                             maxDistanceFromBoundary, minAlignedMarkerCount, minAlignedFraction, maxSkip, maxDrift, maxTrim,
                             maxBand, matchScore, mismatchScore, gapScore):

@@ -540,3 +540,59 @@ def _records_to_array(ptr, n):
         return np.zeros((0, 3), np.uint32)
     # No copy: the library writes the third word as 0 / 1 (byte 0 = isSameStrand, padding bytes zero).
     return _owned_array(ptr, 3 * n, np.uint32).reshape(n, 3)
+
+
+# ---- flagPalindromicReads (shb_flag_palindromic_reads) ---------------------------------------------------------------
+class PalindromicParams(C.Structure):
+    """shb_palindromic_params: the arguments of Assembler::flagPalindromicReads (threadCount is ignored)."""
+    _fields_ = [("maxSkip", C.c_uint32), ("maxDrift", C.c_uint32), ("maxMarkerFrequency", C.c_uint32), ("deltaThreshold", C.c_uint32),
+                ("alignedFractionThreshold", C.c_double), ("nearDiagonalFractionThreshold", C.c_double), ("threadCount", C.c_uint64)]
+
+
+class PalindromicResult(C.Structure):
+    _fields_ = [("readCount", C.c_uint64), ("palindromicReadCount", C.c_uint64), ("exactReadCount", C.c_uint64),
+                ("vertexCount", C.c_uint64), ("edgeCount", C.c_uint64), ("heapPushCount", C.c_uint64),
+                ("heapsortFallbackCount", C.c_uint64), ("totalMs", C.c_double), ("exactMs", C.c_double),
+                ("kernelLaunches", C.c_uint64)]
+
+    def asdict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+def make_palindromic_params(maxSkip=100, maxDrift=100, maxMarkerFrequency=10, alignedFractionThreshold=0.1,
+                            nearDiagonalFractionThreshold=0.1, deltaThreshold=100, threadCount=0):
+    return PalindromicParams(maxSkip=int(maxSkip), maxDrift=int(maxDrift), maxMarkerFrequency=int(maxMarkerFrequency),
+                             deltaThreshold=int(deltaThreshold), alignedFractionThreshold=float(alignedFractionThreshold),
+                             nearDiagonalFractionThreshold=float(nearDiagonalFractionThreshold), threadCount=int(threadCount))
+
+
+def flag_palindromic_reads(ctx: Context, params: PalindromicParams, read_flags=None, want_counts=True):
+    """Flags palindromic reads on the markers ctx holds. read_flags (uint8[R], optional) is updated in place (bit 0 only).
+    Returns (aligned uint32[R] or None, nearDiagonal uint32[R] or None, PalindromicResult). For reads decided without an
+    alignment the counts are the prefilter's bounds (see include/shasta_b200.h)."""
+    L = lib()
+    f = L.shb_flag_palindromic_reads
+    f.argtypes = [C.c_void_p, C.POINTER(PalindromicParams), C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PalindromicResult)]
+    R = ctx.read_count
+    aligned = np.zeros(R, np.uint32) if want_counts else None
+    near = np.zeros(R, np.uint32) if want_counts else None
+    if read_flags is not None:
+        assert read_flags.dtype == np.uint8 and read_flags.flags["C_CONTIGUOUS"] and len(read_flags) == R
+    res = PalindromicResult()
+    _check(f(ctx._h, C.byref(params), None if read_flags is None else read_flags.ctypes.data,
+             None if aligned is None else aligned.ctypes.data, None if near is None else near.ctypes.data, C.byref(res)))
+    return aligned, near, res
+
+
+def palindromic_read_alignment(ctx: Context, read_id, params: PalindromicParams):
+    """The alignment of read_id against its reverse complement (method 0). Returns ordinals uint32[n,2]."""
+    L = lib()
+    f = L.shb_palindromic_read_alignment
+    f.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(PalindromicParams), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
+    ords = C.c_void_p()
+    n = C.c_uint64()
+    _check(f(ctx._h, int(read_id), C.byref(params), C.byref(ords), C.byref(n)))
+    out = np.ctypeslib.as_array(C.cast(ords, C.POINTER(C.c_uint32)), (n.value, 2)).copy() if n.value else np.zeros((0, 2), np.uint32)
+    if ords:
+        L.shb_free(ords)
+    return out

@@ -40,6 +40,9 @@ void computeCandidateTable(shb_context* c, const void* candidates, uint64_t n, u
 void createReadGraph(shb_context* c, void* alignmentData, uint64_t n, uint64_t readCount, uint32_t maxAlignmentCount,
                      const uint8_t* eligibleHost,
                      uint8_t** keepOut, void** edgesOut, uint64_t* edgeCountOut, uint32_t** connectivityTocOut, uint32_t** connectivityDataOut);
+void flagPalindromicReads(shb_context* c, const shb_palindromic_params& p, uint8_t* flagsOut, uint32_t* alignedOut,
+                          uint32_t* nearOut, shb_palindromic_result* result);
+void palindromicReadAlignment(shb_context* c, uint64_t readId, const shb_palindromic_params& p, uint32_t** ordinals, uint64_t* count);
 void readGraph2Criteria(const uint32_t* rec, uint64_t n, const double* percentiles, shb_read_graph2_criteria& out, std::vector<uint8_t>& eligible);
 
 template<class F> shb_status guarded(F&& f)
@@ -427,6 +430,25 @@ shb_status shb_create_read_graph2(shb_context* c, void* alignmentData, uint64_t 
         eligible.push_back(0);      // never an empty array
         createReadGraph(c, alignmentData, alignmentCount, readCount, maxAlignmentCount, eligible.data(), keep, edges, edgeCount,
                         connectivityToc, connectivityData);
+    });
+}
+
+shb_status shb_flag_palindromic_reads(shb_context* c, const shb_palindromic_params* params, uint8_t* readFlags,
+                                      uint32_t* alignedMarkerCount, uint32_t* nearDiagonalMarkerCount,
+                                      shb_palindromic_result* result)
+{
+    return guarded([&] {
+        SHB_REQUIRE(c && params, SHB_ERR_INVALID, "Null argument.");
+        flagPalindromicReads(c, *params, readFlags, alignedMarkerCount, nearDiagonalMarkerCount, result);
+    });
+}
+
+shb_status shb_palindromic_read_alignment(shb_context* c, uint64_t readId, const shb_palindromic_params* params,
+                                          uint32_t** ordinals, uint64_t* count)
+{
+    return guarded([&] {
+        SHB_REQUIRE(c && params && ordinals && count, SHB_ERR_INVALID, "Null argument.");
+        palindromicReadAlignment(c, readId, *params, ordinals, count);
     });
 }
 
