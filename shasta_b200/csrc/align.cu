@@ -67,19 +67,7 @@ DpLaunch dpLaunch(const DpClass& k, uint32_t jobs)
     return DpLaunch{ceilDiv(jobs, warps * (32 / k.lanes)), warps * 32, smemForClass(k, warps)};
 }
 
-// Stage 1 with a trace / stage 2: the kernel instantiation of band class k.
-template<uint32_t K = 0, class... Args> void launchStage1(uint32_t k, const DpLaunch& l, cudaStream_t st, Args... args)
-{
-    if constexpr(K < kDpClassCount) {
-        if(k != K) { launchStage1<K + 1>(k, l, st, args...); return; }
-        constexpr DpClass cl = dpClassAt(K);
-        if constexpr(cl.c == 0) {
-            SHB_CUDA(cudaFuncSetAttribute(method3Stage1Kernel<32, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, int(scanKernelSmemLimit())));
-        }
-        auto* kernel = &method3Stage1Kernel<int(cl.lanes), int(cl.c)>;
-        SHB_LAUNCH(kernel, l.blocks, l.threads, l.smem, st, args...);
-    }
-}
+// The banded DP kernel instantiation of band class k.
 template<uint32_t K = 0, class... Args> void launchBanded(uint32_t k, const DpLaunch& l, cudaStream_t st, Args... args)
 {
     if constexpr(K < kDpClassCount) {
@@ -407,6 +395,45 @@ void buildClassOrder(AlignWorker& w, const DpJob* jobs, uint32_t nJobs, std::vec
     for(size_t k = 0; k < classCounts.size(); k++) classCounts[k] = h[k];
 }
 
+// Runs the jobs of b.order class by class (classCounts from buildClassOrder), in chunks of at most chunkMax jobs.
+// Band class k sits at index firstBanded + k: the DP of a chunk (group per job) on its stream, then its traceback (thread
+// per job) and equal-k-mer filter (warp per job) on a high-priority stream. The classes below firstBanded (the forward
+// classes of method 3's stage 1) go to launchOther(k, count, order, stream). The main stream continues after all of them.
+// trace, endCells, runs, runCounts, ordinals and counts must be reserved for the jobs.
+template<class F> void runDpClasses(AlignWorker& w, const std::vector<uint64_t>& classCounts, uint32_t chunkMax, uint32_t firstBanded,
+                                    const DpJob* jobs, const uint32_t* sequences, DpScores scores, F launchOther)
+{
+    Batch& b = w.batch;
+    BandedArgs g;
+    g.kmerIds = sequences; g.scores = scores; g.fma = FmaUnits{1, 2, 4};
+    size_t unit = 0;
+    forEachClassConcurrently(w, classCounts, chunkMax, [&](int k, uint32_t count, uint64_t offset, cudaStream_t s) {
+        const uint32_t* order = b.order + offset;
+        if(uint32_t(k) < firstBanded) { launchOther(uint32_t(k), count, order, s); return; }
+        const uint32_t cls = uint32_t(k) - firstBanded;
+        BandedArgs gk = g;
+        gk.n = count; gk.order = order; gk.wMax = dpClassAt(cls).wMax;
+        launchBanded(cls, dpLaunch(dpClassAt(cls), count), s, gk, jobs, b.trace.get(), b.endCells.get());
+        if(unit == w.unitEvents.size()) {
+            cudaEvent_t e = nullptr;
+            SHB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+            w.unitEvents.push_back(e);
+        }
+        SHB_CUDA(cudaEventRecord(w.unitEvents[unit], s));
+        cudaStream_t hs = w.hiStream[unit % AlignWorker::kHiStreams];
+        SHB_CUDA(cudaStreamWaitEvent(hs, w.unitEvents[unit], 0));
+        unit++;
+        SHB_LAUNCH(tracebackKernel, ceilDiv(count, 128), 128, 0, hs, count, order, jobs, (const int2*)b.endCells.get(),
+                   (const uint32_t*)b.trace.get(), b.runs.get(), b.runCounts.get());
+        SHB_LAUNCH(filterStepsKernel, ceilDiv(count, 4), 128, 0, hs, count, order, jobs, sequences,
+                   (const uint2*)b.runs.get(), (const uint32_t*)b.runCounts.get(), b.ordinals.get(), b.counts.get());
+    });
+    for(size_t i = 0; i < std::min<size_t>(unit, AlignWorker::kHiStreams); i++) {
+        SHB_CUDA(cudaEventRecord(w.hiJoinEv[i], w.hiStream[i]));
+        SHB_CUDA(cudaStreamWaitEvent(w.stream, w.hiJoinEv[i], 0));
+    }
+}
+
 // Scratch offsets + the banded DP + traceback for nJobs jobs whose lo/hi/state are set.
 void runBandedJobs(AlignWorker& w, uint32_t nJobs, const uint32_t* sequences, DpScores scores)
 {
@@ -429,34 +456,9 @@ void runBandedJobs(AlignWorker& w, uint32_t nJobs, const uint32_t* sequences, Dp
     SHB_CUDA(cudaMemsetAsync(b.counts.get(), 0, 4ull * nJobs, st));
     std::vector<uint64_t> classCounts;
     buildClassOrder(w, b.jobs.get(), nJobs, classCounts);
-    BandedArgs g;
-    g.kmerIds = sequences; g.scores = scores; g.fma = FmaUnits{1, 2, 4};
     SHB_CUDA(cudaEventRecord(w.dp2a, st));
-    // Per chunk: DP (warp per job) on its stream, then traceback (thread per job) and equal-k-mer filter (warp per job)
-    // on a high-priority stream.
-    size_t unit = 0;
-    forEachClassConcurrently(w, classCounts, envCount("SHB_ALIGN_CHUNK", 32768), [&](int k, uint32_t count, uint64_t offset, cudaStream_t s) {
-        BandedArgs gk = g;
-        gk.n = count; gk.order = b.order + offset; gk.wMax = dpClassAt(k).wMax;
-        launchBanded(uint32_t(k), dpLaunch(dpClassAt(k), count), s, gk, (const DpJob*)b.jobs.get(), b.trace.get(), b.endCells.get());
-        if(unit == w.unitEvents.size()) {
-            cudaEvent_t e = nullptr;
-            SHB_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-            w.unitEvents.push_back(e);
-        }
-        SHB_CUDA(cudaEventRecord(w.unitEvents[unit], s));
-        cudaStream_t hs = w.hiStream[unit % AlignWorker::kHiStreams];
-        SHB_CUDA(cudaStreamWaitEvent(hs, w.unitEvents[unit], 0));
-        unit++;
-        SHB_LAUNCH(tracebackKernel, ceilDiv(count, 128), 128, 0, hs, count, gk.order, (const DpJob*)b.jobs.get(),
-                   (const int2*)b.endCells.get(), (const uint32_t*)b.trace.get(), b.runs.get(), b.runCounts.get());
-        SHB_LAUNCH(filterStepsKernel, ceilDiv(count, 4), 128, 0, hs, count, gk.order, (const DpJob*)b.jobs.get(), sequences,
-                   (const uint2*)b.runs.get(), (const uint32_t*)b.runCounts.get(), b.ordinals.get(), b.counts.get());
-    });
-    for(size_t i = 0; i < std::min<size_t>(unit, AlignWorker::kHiStreams); i++) {
-        SHB_CUDA(cudaEventRecord(w.hiJoinEv[i], w.hiStream[i]));
-        SHB_CUDA(cudaStreamWaitEvent(st, w.hiJoinEv[i], 0));
-    }
+    runDpClasses(w, classCounts, envCount("SHB_ALIGN_CHUNK", 32768), 0, b.jobs.get(), sequences, scores,
+                 [](uint32_t, uint32_t, const uint32_t*, cudaStream_t) {});
     SHB_CUDA(cudaEventRecord(w.dp2b, st));
 }
 
@@ -590,33 +592,38 @@ void processBatch(AlignCall& call, AlignWorker& w, uint64_t begin, uint32_t nb, 
             const unsigned long long traceWords1 = readBack<unsigned long long>(total64, st);
             b.trace.reserve(traceWords1 + 1);
             w.traceWords += traceWords1;
-            SHB_LAUNCH(setTraceOffsetsKernel, ceilDiv(nb, 256), 256, 0, st, b.jobs1.get(), nb, (const unsigned long long*)b.twOff.get(),
-                       (const unsigned long long*)nullptr);
-            // Ordinal slots (also the stage-1 path scratch): offsets must be in jobs[] before stage 1 runs.
+            // The jobs too long for the forward kernel keep their path's runs and kept steps in the candidate's stage-2
+            // ordinal slots (min(nx, ny) is at least the number of downsampled diagonal steps).
             b.outOff.reserve(nb);
             exclusiveScan<unsigned long long>(b.outCnt.get(), b.outOff.get(), nb, total64, b.scanWs64.get(), st);
             const unsigned long long slots1 = readBack<unsigned long long>(total64, st);
-            b.ordinals.reserve(slots1 + 1);
-            SHB_LAUNCH(setOutOffsetsKernel, ceilDiv(nb, 256), 256, 0, st, b.jobs.get(), nb, (const unsigned long long*)b.outOff.get());
+            b.ordinals.reserve(slots1 + 1); b.runs.reserve(slots1 + 1);
+            b.counts.reserve(nb); b.endCells.reserve(nb); b.runCounts.reserve(nb);
+            SHB_LAUNCH(setTraceOffsetsKernel, ceilDiv(nb, 256), 256, 0, st, b.jobs1.get(), nb, (const unsigned long long*)b.twOff.get(),
+                       (const unsigned long long*)b.outOff.get());
             Method3Args g1;
             g1.candidates = b.cand.get(); g1.candidateBegin = begin; g1.n = nb;
             g1.toc = c->toc.get(); g1.dsToc = ac.dsToc.get(); g1.dsKmer = ac.dsKmer.get(); g1.dsOrdinal = ac.dsOrdinal.get();
-            g1.scores = call.scores; g1.fma = FmaUnits{1, 2, 4}; g1.bandExtend = o.bandExtend; g1.maxBand = o.maxBand;
+            g1.scores = call.scores; g1.bandExtend = o.bandExtend; g1.maxBand = o.maxBand;
             std::vector<uint64_t> classCounts1;
             buildClassOrder(w, b.jobs1.get(), nb, classCounts1, true);
             SHB_CUDA(cudaEventRecord(w.dp1a, st));
-            forEachClassConcurrently(w, classCounts1, 0xffffffffu, [&](int k, uint32_t count, uint64_t offset, cudaStream_t s) {
+            // One launch per class: cutting stage 1 into SHB_ALIGN_CHUNK chunks measured slower on long reads
+            // (bench.py --workload nanopore-ul-20k).
+            runDpClasses(w, classCounts1, 0xffffffffu, kDpForwardClassCount, b.jobs1.get(), ac.dsKmer.get(), call.scores,
+                         [&](uint32_t k, uint32_t count, const uint32_t* order, cudaStream_t s) {
                 Method3Args gk = g1;
-                gk.n = count; gk.order = b.order + offset;
-                if(uint32_t(k) < kDpForwardClassCount) {
-                    gk.wMax = 0;
-                    launchStage1Forward(uint32_t(k), count, s, gk, (const DpJob*)b.jobs1.get(), b.jobs.get());
-                    return;
-                }
-                const uint32_t cls = uint32_t(k) - kDpForwardClassCount;   // too long for the forward kernel: DP with a trace
-                gk.wMax = dpClassAt(cls).wMax;
-                launchStage1(cls, dpLaunch(dpClassAt(cls), count), s, gk, b.jobs1.get(), b.trace.get(), b.jobs.get(), b.ordinals.get());
+                gk.n = count; gk.order = order;
+                launchStage1Forward(k, count, s, gk, (const DpJob*)b.jobs1.get(), b.jobs.get());
             });
+            // The band of the jobs that took the trace path: they follow the forward classes in b.order.
+            uint64_t forwardJobs = 0, tracedJobs = 0;
+            for(uint32_t k = 0; k < classCounts1.size(); k++) (k < kDpForwardClassCount ? forwardJobs : tracedJobs) += classCounts1[k];
+            if(tracedJobs) {
+                SHB_LAUNCH(stage1BandKernel, ceilDiv(tracedJobs, 4), 128, 0, st, uint32_t(tracedJobs), b.order + forwardJobs,
+                           (const DpJob*)b.jobs1.get(), (const uint32_t*)ac.dsOrdinal.get(), (const uint2*)b.ordinals.get(),
+                           (const uint32_t*)b.runCounts.get(), (const uint32_t*)b.counts.get(), o.bandExtend, o.maxBand, b.jobs.get());
+            }
             SHB_CUDA(cudaEventRecord(w.dp1b, st));
             stage1Timed = true;
             if(getenv("SHB_TRACE") && begin == 0) {        // band-width and active-column statistics of the first batch
