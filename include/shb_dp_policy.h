@@ -17,8 +17,11 @@
  *
  * This header is included by BOTH the CUDA kernels (shasta_b200/csrc/align_kernels.cuh) and the CPU oracle
  * (oracle/align_oracle.c), so a later check against real SeqAn touches this file only (build both with e.g.
- * -DSHB_DP_VERT_BEFORE_HORZ=0). The oracle can additionally switch policy at run time (orc_set_dp_policy) to measure how
- * many candidate pairs are exposed to the choice at all (bench.py: "policy_invariant_fraction").
+ * -DSHB_DP_VERT_BEFORE_HORZ=0). That switch is tested: build() also compiles the library under each of the seven other
+ * policies (`make -C shasta_b200/csrc policies`: shasta_b200/lib/dp_policy/libshasta_b200_policy<N>.so, N = the bits
+ * below), and tests/test_gpu_dp_policies.py holds every policy's kernels to the oracle under the same policy. The oracle
+ * can additionally switch policy at run time (orc_set_dp_policy) to measure how many candidate pairs are exposed to the
+ * choice at all (bench.py: "policy_invariant_fraction").
  */
 #ifndef SHB_DP_POLICY_H
 #define SHB_DP_POLICY_H

@@ -708,9 +708,11 @@ method3Stage1ForwardKernel(Method3Args g, const DpJob* __restrict__ jobs1, DpJob
                 vH = h; vP = pr;
                 H[r] = h; P[r] = pr;
             }
-            // End-cell candidates: row ny in every column, then every row of column nx (column-major order; the boundary
-            // cells score 0 and come first, so only positive scores can win under the first-maximum rule).
-            if(lane == lastLane) {
+            // End-cell candidates in column-major order: row ny of the columns before nx, then every row of column nx (the
+            // cell (nx, ny) is visited once, after the rows below it). The boundary cell (0, ny) scores 0 and comes
+            // first: the start value (score 0, no cell) stands for it, so under the first-maximum rule only positive scores
+            // win. The boundary cell (nx, 0) comes after the row-ny cells of the columns before nx: see below the loop.
+            if(lane == lastLane && i != nx) {
                 int32_t h = 0; uint32_t pr = 0;
                 switch(rLast) {                  // group-uniform; a jump instead of R selects per value
 #define SHB_PICK_ROW(k) case k: if constexpr(k < R) { h = H[k]; pr = P[k]; } break;
@@ -730,6 +732,12 @@ method3Stage1ForwardKernel(Method3Args g, const DpJob* __restrict__ jobs1, DpJob
             }
         }
         upH = inH; upP = inP;
+    }
+    if constexpr(!SHB_DP_END_FIRST_MAX) {
+        // Under the last-maximum rule the boundary cell (nx, 0) (score 0, empty path) wins a tie with a row-ny cell of an
+        // earlier column. It joins here, after the per-lane updates above (whose >= would let such a row-ny cell replace
+        // it), and the reduction below orders it among the lanes' candidates.
+        if(lane == 0 && dpEndCellBetter(0, nx, 0, bestScore, bestI, bestJ)) { bestScore = 0; bestI = nx; bestJ = 0; bestP = kPairNoDiagonalStep; }
     }
     // Maximum score, then the visiting order of the end-cell rule (over the lanes of the group).
 #pragma unroll
