@@ -357,6 +357,60 @@ shb_status shb_create_read_graph2(shb_context* ctx, void* alignmentData, uint64_
                                   shb_read_graph2_criteria* criteria, uint8_t** keep, void** edges, uint64_t* edgeCount,
                                   uint32_t** connectivityToc, uint32_t** connectivityData);
 
+// ---- createMarkerGraphVertices (src/AssemblerMarkerGraph.cpp:38-770) ------------------------------------------------
+// The arguments of Assembler::createMarkerGraphVertices (defaults src/AssemblerOptions.cpp:577-685: 10, 100, 0, 0, 0.08,
+// 2). minCoverage 0 selects it from the disjoint-set size histogram with the reference's PeakFinder. threadCount is
+// accepted and ignored.
+typedef struct {
+    uint64_t minCoverage, maxCoverage, minCoveragePerStrand;
+    uint64_t allowDuplicateMarkers;         // 0 / 1
+    double peakFinderMinAreaFraction;
+    uint64_t peakFinderAreaStartIndex;
+    uint64_t threadCount;
+} shb_marker_graph_params;
+typedef struct {
+    uint64_t markerCount;
+    uint64_t minCoverageUsed;               // Assembler::markerGraphMinCoverageUsed
+    uint64_t peakFinderFailed;              // 1: the reference's PeakFinder throws here, minCoverage 5 was used
+    double peakFinderObservedAreaFraction;  // PeakFinderException::observedPercentArea when it does
+    uint64_t edgePairsUsed, edgePairsSkipped;   // skipped: crossesStrands, hasInconsistentAlignment or a chimeric read
+    uint64_t alignedMarkerPairs;            // ordinal pairs decoded from the used alignments (two unions each)
+    uint64_t disjointSetCount, keptDisjointSetCount, badDisjointSetCount, vertexCount;
+    uint64_t histogramSize;                 // entries of *histogram: largest set size + 1 (0 without markers)
+    uint64_t peakDeviceBytes;               // high-water mark of the device memory this call allocated (its own buffers and
+                                            // the growth of the context's radix-sort workspace)
+    double deviceMs, totalMs;               // device time line from the first to the last kernel; wall time of the call
+    uint64_t kernelLaunches;
+} shb_marker_graph_result;
+/* Replaces Assembler::createMarkerGraphVertices on the markers held by ctx (every read: a context that holds a read range
+ * returns SHB_ERR_STATE). Vertices are numbered in increasing order of their smallest marker id (the reference's order
+ * depends on thread scheduling); the partition, each vertex's markers, the histogram and the counts are the reference's.
+ *   readGraphEdges  : edgeCount 16-byte ReadGraphEdge records (Data/ReadGraphEdges payload), pairs (i, i+1), i even.
+ *   compressedToc   : uint64[alignmentCount+1], compressedData: Data/CompressedAlignments payload.
+ *   readFlags       : uint8[R] as in Data/ReadFlags (bit 1 = isChimeric) at call time.
+ *   vertexTable     : receives Uint40[M] (5 bytes each, 2^40-1 = no vertex) = Data/MarkerGraphVertexTable payload.
+ *   verticesToc     : receives Uint40[V+1]; verticesData: uint64[toc[V]] (= Data/MarkerGraphVertices.{toc,data}).
+ *   histogram       : receives uint64[result->histogramSize]: the number of disjoint sets of each size.
+ * Free the four arrays with shb_free. Inputs that trip one of the reference's assertions return SHB_ERR_INVALID (odd edge
+ * count, a pair that is not an edge and its reverse complement, unordered oriented read ids, an alignmentId out of range,
+ * aligned markers with different k-mer ids, and, beyond the reference's checks, a malformed compressed alignment). */
+shb_status shb_create_marker_graph_vertices(shb_context* ctx, const shb_marker_graph_params* params, const void* readGraphEdges,
+                                            uint64_t edgeCount, const uint64_t* compressedToc, const uint8_t* compressedData,
+                                            uint64_t alignmentCount, const uint8_t* readFlags, uint8_t** vertexTable,
+                                            uint8_t** verticesToc, uint64_t** verticesData, uint64_t** histogram,
+                                            shb_marker_graph_result* result);
+/* Replaces Assembler::findMarkerGraphReverseComplementVertices (:1134-1230) for vertices in any numbering (the reference's
+ * own files included): rcVertex receives uint64[vertexCount], free with shb_free. A vertex whose reverse complemented
+ * markers are not all on one vertex, or whose reverse complement's reverse complement is not itself, returns
+ * SHB_ERR_INVALID. */
+shb_status shb_find_marker_graph_reverse_complement_vertices(shb_context* ctx, const uint8_t* vertexTable, const uint8_t* verticesToc,
+                                                             const uint64_t* verticesData, uint64_t vertexCount, uint64_t** rcVertex);
+/* PeakFinder::findPeaks + findXCutoff (src/PeakFinder.cpp:23-198) on a histogram of n entries, host only. Returns 1 where
+ * the reference throws PeakFinderException (*observedAreaFraction = its observedPercentArea), else 0 with *cutoff. n = 0,
+ * undefined in the reference, returns 1 with observed area 0. */
+int shb_peak_finder_cutoff(const uint64_t* histogram, uint64_t n, double minAreaFraction, uint64_t startIndex, uint64_t* cutoff,
+                           double* observedAreaFraction);
+
 /* ------------------------------------------------------------------------------------------
  * Read-sharded multi-GPU runs (SURVEY.md section 8e; BASELINE.json configs[2..4]): one process (and one context) per GPU,
  * NCCL over NVLink / NVSwitch for the two exchanges LowHash0 needs (bucket entries per iteration, pair counts once) and

@@ -400,3 +400,80 @@ class Assembler:
         mm_write_vector_of_vectors(self._name("CompressedAlignments"), ctoc, cdata, data_object_size=1, page_size=self.page_size)
         mm_write_vector_of_vectors(self._name("AlignmentTable"), ttoc, tdata, data_object_size=4, toc_dtype=np.uint32,
                                    page_size=self.page_size)
+
+    # ------------------------------------------------------------------ marker graph vertices
+    def accessReadGraph(self):
+        """Data/ReadGraphEdges: 16-byte ReadGraphEdge records (src/ReadGraph.hpp:37-57)."""
+        self._read_graph_edges = np.asarray(mm_read_vector(self._name("ReadGraphEdges"), np.uint32, object_size=16)).reshape(-1, 4)
+
+    def createMarkerGraphVertices(self, minCoverage, maxCoverage, minCoveragePerStrand, allowDuplicateMarkers,
+                                  peakFinderMinAreaFraction, peakFinderAreaStartIndex, threadCount=0):
+        """Assembler::createMarkerGraphVertices (src/AssemblerMarkerGraph.cpp:38-518, binding src/PythonModule.cpp:428-436).
+        Writes Data/MarkerGraphVertexTable (Uint40 per marker), Data/MarkerGraphVertices.{toc,data} (VectorOfVectors<MarkerId,
+        Uint40>) and DisjointSetsHistogram.csv, and prints the reference's lines. Vertices are numbered in increasing order of
+        their first marker. Data/ReadFlags is read now: flagChimericReads may have changed it. threadCount is ignored."""
+        from . import capi
+        self.checkMarkersAreOpen()
+        edges = getattr(self, "_read_graph_edges", None)
+        if edges is None and getattr(self, "_read_graph", None) is not None:
+            edges = self._read_graph[0]                 # created in this session by createReadGraph / createReadGraph2
+        if edges is None:
+            raise RuntimeError("Read graph is not accessible.")
+        if self._compressed is None:
+            raise RuntimeError("Compressed alignments are not accessible.")
+        ctx = self._upload_markers()
+        flags = np.asarray(mm_read_vector(self._name("ReadFlags"), np.uint8, object_size=1))
+        params = capi.make_marker_graph_params(minCoverage, maxCoverage, minCoveragePerStrand, allowDuplicateMarkers,
+                                               peakFinderMinAreaFraction, peakFinderAreaStartIndex, threadCount)
+        try:
+            table, vtoc, vdata, hist, res = capi.create_marker_graph_vertices(ctx, params, edges, self._compressed[0],
+                                                                              self._compressed[1], flags)
+        except capi.ShastaB200Error as e:
+            raise RuntimeError(str(e)) from None
+        write_disjoint_sets_histogram_csv("DisjointSetsHistogram.csv", hist)
+        if minCoverage == 0:
+            if res.peakFinderFailed:
+                print("Unable to automatically select MarkerGraph.minCoverage. No significant cutoff found in disjoint sets size "
+                      f"distribution. Observed peak has percent total area of {_ostream_double(res.peakFinderObservedAreaFraction)}\n"
+                      f"minPercentArea is {_ostream_double(peakFinderMinAreaFraction)}\n"
+                      f"See DisjointSetsHistogram.csv.Using MarkerGraph.minCoverage = {res.minCoverageUsed}")
+            else:
+                print(f"Automatically selected value of MarkerGraph.minCoverage is {res.minCoverageUsed}")
+        print(f"Kept {res.keptDisjointSetCount} disjoint sets with coverage in the requested range.")
+        print(f"Found {res.badDisjointSetCount} disjoint sets with more than one marker on a single oriented read or with less than "
+              f"{minCoveragePerStrand} supporting oriented reads on each strand.")
+        self.markerGraphMinCoverageUsed = res.minCoverageUsed
+        self._marker_graph = (table, vtoc, vdata)
+        mm_write_vector(self._name("MarkerGraphVertexTable"), table, object_size=5, page_size=self.page_size)
+        mm_write_vector(self._name("MarkerGraphVertices.toc"), vtoc, object_size=5, page_size=self.page_size)
+        mm_write_vector(self._name("MarkerGraphVertices.data"), vdata, object_size=8, page_size=self.page_size)
+
+    def accessMarkerGraphVertices(self, readWriteAccess=False):
+        """Data/MarkerGraphVertexTable and Data/MarkerGraphVertices.{toc,data} (src/AssemblerMarkerGraph.cpp)."""
+        table = mm_read_vector(self._name("MarkerGraphVertexTable"), np.uint8, object_size=5)
+        vtoc = mm_read_vector(self._name("MarkerGraphVertices.toc"), np.uint8, object_size=5)
+        vdata = mm_read_vector(self._name("MarkerGraphVertices.data"), np.uint64, object_size=8)
+        self._marker_graph = (np.asarray(table), np.asarray(vtoc), np.asarray(vdata))
+
+    def findMarkerGraphReverseComplementVertices(self, threadCount=0):
+        """Assembler::findMarkerGraphReverseComplementVertices (:1134-1230). Writes Data/MarkerGraphReverseComplementeVertex
+        (the reference's file name), uint64 per vertex. Works on vertices in any numbering, the reference's included."""
+        from . import capi
+        if getattr(self, "_marker_graph", None) is None:
+            raise RuntimeError("Marker graph vertices are not accessible.")
+        ctx = self._upload_markers()
+        table, vtoc, vdata = self._marker_graph
+        try:
+            rc = capi.find_marker_graph_reverse_complement_vertices(ctx, table, vtoc, vdata)
+        except capi.ShastaB200Error as e:
+            raise RuntimeError(str(e)) from None
+        mm_write_vector(self._name("MarkerGraphReverseComplementeVertex"), rc, object_size=8, page_size=self.page_size)
+
+
+def write_disjoint_sets_histogram_csv(path, histogram):
+    """DisjointSetsHistogram.csv as createMarkerGraphVertices writes it (src/AssemblerMarkerGraph.cpp:224-231): nonzero rows."""
+    with open(path, "w") as csv:
+        csv.write("Coverage,Frequency\n")
+        for coverage, frequency in enumerate(np.asarray(histogram, np.uint64).tolist()):
+            if frequency:
+                csv.write(f"{coverage},{frequency}\n")

@@ -596,3 +596,93 @@ def palindromic_read_alignment(ctx: Context, read_id, params: PalindromicParams)
     if ords:
         L.shb_free(ords)
     return out
+
+
+# ---- createMarkerGraphVertices (shb_create_marker_graph_vertices) ----------------------------------------------------
+class MarkerGraphParams(C.Structure):
+    """shb_marker_graph_params: the arguments of Assembler::createMarkerGraphVertices (threadCount is ignored)."""
+    _fields_ = [("minCoverage", C.c_uint64), ("maxCoverage", C.c_uint64), ("minCoveragePerStrand", C.c_uint64),
+                ("allowDuplicateMarkers", C.c_uint64), ("peakFinderMinAreaFraction", C.c_double),
+                ("peakFinderAreaStartIndex", C.c_uint64), ("threadCount", C.c_uint64)]
+
+
+class MarkerGraphResult(C.Structure):
+    _fields_ = [("markerCount", C.c_uint64), ("minCoverageUsed", C.c_uint64), ("peakFinderFailed", C.c_uint64),
+                ("peakFinderObservedAreaFraction", C.c_double), ("edgePairsUsed", C.c_uint64), ("edgePairsSkipped", C.c_uint64),
+                ("alignedMarkerPairs", C.c_uint64), ("disjointSetCount", C.c_uint64), ("keptDisjointSetCount", C.c_uint64),
+                ("badDisjointSetCount", C.c_uint64), ("vertexCount", C.c_uint64), ("histogramSize", C.c_uint64),
+                ("peakDeviceBytes", C.c_uint64), ("deviceMs", C.c_double), ("totalMs", C.c_double), ("kernelLaunches", C.c_uint64)]
+
+    def asdict(self):
+        return {k: getattr(self, k) for k, _ in self._fields_}
+
+
+def make_marker_graph_params(minCoverage=10, maxCoverage=100, minCoveragePerStrand=0, allowDuplicateMarkers=False,
+                             peakFinderMinAreaFraction=0.08, peakFinderAreaStartIndex=2, threadCount=0):
+    """Defaults of src/AssemblerOptions.cpp:577-685."""
+    return MarkerGraphParams(int(minCoverage), int(maxCoverage), int(minCoveragePerStrand), int(bool(allowDuplicateMarkers)),
+                             float(peakFinderMinAreaFraction), int(peakFinderAreaStartIndex), int(threadCount))
+
+
+def uint40_to_uint64(a):
+    """Uint40 little-endian records (uint8[5n]) -> uint64[n]."""
+    b = np.asarray(a, np.uint8).reshape(-1, 5)
+    out = np.zeros((len(b), 8), np.uint8)
+    out[:, :5] = b
+    return out.view(np.uint64).reshape(-1)
+
+
+def uint64_to_uint40(a):
+    return np.ascontiguousarray(np.asarray(a, np.uint64).reshape(-1, 1).view(np.uint8)[:, :5]).reshape(-1)
+
+
+def create_marker_graph_vertices(ctx: Context, params: MarkerGraphParams, edges, compressed_toc, compressed_data, read_flags):
+    """Assembler::createMarkerGraphVertices on the markers ctx holds. edges: uint32[E,4] ReadGraphEdge records.
+    Returns (vertexTable uint8[5M] (Uint40), verticesToc uint8[5(V+1)] (Uint40), verticesData uint64[], histogram uint64[],
+    MarkerGraphResult)."""
+    L = lib()
+    f = L.shb_create_marker_graph_vertices
+    f.argtypes = [C.c_void_p, C.POINTER(MarkerGraphParams), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
+                  C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                  C.POINTER(MarkerGraphResult)]
+    e = np.ascontiguousarray(edges, np.uint32).reshape(-1, 4)
+    t = np.ascontiguousarray(compressed_toc, np.uint64)
+    d = np.ascontiguousarray(compressed_data, np.uint8)
+    fl = np.ascontiguousarray(read_flags, np.uint8)
+    table, vtoc, vdata, hist = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
+    res = MarkerGraphResult()
+    _check(f(ctx._h, C.byref(params), _ptr(e), len(e), _ptr(t), _ptr(d), len(t) - 1, _ptr(fl), C.byref(table), C.byref(vtoc),
+             C.byref(vdata), C.byref(hist), C.byref(res)))
+    V = res.vertexCount
+    tocn = _owned_array(vtoc, 5 * (V + 1), np.uint8)
+    n = int(uint40_to_uint64(tocn)[-1]) if V else 0
+    if not V:
+        tocn = np.zeros(5, np.uint8)
+    return (_owned_array(table, 5 * res.markerCount, np.uint8), tocn, _owned_array(vdata, n, np.uint64),
+            _owned_array(hist, res.histogramSize, np.uint64), res)
+
+
+def find_marker_graph_reverse_complement_vertices(ctx: Context, vertex_table, vertices_toc, vertices_data):
+    """Assembler::findMarkerGraphReverseComplementVertices. vertex_table / vertices_toc: Uint40 bytes. Returns uint64[V]."""
+    L = lib()
+    f = L.shb_find_marker_graph_reverse_complement_vertices
+    f.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_void_p)]
+    t = np.ascontiguousarray(vertex_table, np.uint8)
+    vt = np.ascontiguousarray(vertices_toc, np.uint8)
+    vd = np.ascontiguousarray(vertices_data, np.uint64)
+    V = len(vt) // 5 - 1
+    rc = C.c_void_p()
+    _check(f(ctx._h, _ptr(t), _ptr(vt), _ptr(vd), V, C.byref(rc)))
+    return _owned_array(rc, V, np.uint64)
+
+
+def peak_finder_cutoff(histogram, min_area_fraction=0.08, start_index=2):
+    """The library's PeakFinder restatement (host only). Returns (threw, cutoff, observedPercentArea)."""
+    L = lib()
+    f = L.shb_peak_finder_cutoff
+    f.restype = C.c_int
+    f.argtypes = [C.c_void_p, C.c_uint64, C.c_double, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_double)]
+    y = np.ascontiguousarray(histogram, np.uint64)
+    cutoff, observed = C.c_uint64(0), C.c_double(0)
+    threw = f(_ptr(y) if len(y) else None, len(y), float(min_area_fraction), int(start_index), C.byref(cutoff), C.byref(observed))
+    return int(threw), int(cutoff.value), float(observed.value)

@@ -44,6 +44,13 @@ void flagPalindromicReads(shb_context* c, const shb_palindromic_params& p, uint8
                           uint32_t* nearOut, shb_palindromic_result* result);
 void palindromicReadAlignment(shb_context* c, uint64_t readId, const shb_palindromic_params& p, uint32_t** ordinals, uint64_t* count);
 void readGraph2Criteria(const uint32_t* rec, uint64_t n, const double* percentiles, shb_read_graph2_criteria& out, std::vector<uint8_t>& eligible);
+bool peakFinderCutoff(const uint64_t* y, uint64_t n, double minAreaFraction, uint64_t startIndex, uint64_t* cutoff, double* observed);
+void createMarkerGraphVertices(shb_context* c, const shb_marker_graph_params& p, const uint32_t* edges, uint64_t edgeCount,
+                               const uint64_t* ctoc, const uint8_t* cdata, uint64_t alignmentCount, const uint8_t* readFlags,
+                               uint8_t** vertexTableOut, uint8_t** verticesTocOut, uint64_t** verticesDataOut, uint64_t** histogramOut,
+                               shb_marker_graph_result* result);
+void findMarkerGraphReverseComplementVertices(shb_context* c, const uint8_t* table5, const uint8_t* toc5, const uint64_t* vdata,
+                                              uint64_t V, uint64_t** rcOut);
 
 template<class F> shb_status guarded(F&& f)
 {
@@ -450,6 +457,41 @@ shb_status shb_palindromic_read_alignment(shb_context* c, uint64_t readId, const
         SHB_REQUIRE(c && params && ordinals && count, SHB_ERR_INVALID, "Null argument.");
         palindromicReadAlignment(c, readId, *params, ordinals, count);
     });
+}
+
+shb_status shb_create_marker_graph_vertices(shb_context* c, const shb_marker_graph_params* params, const void* readGraphEdges,
+                                            uint64_t edgeCount, const uint64_t* compressedToc, const uint8_t* compressedData,
+                                            uint64_t alignmentCount, const uint8_t* readFlags, uint8_t** vertexTable,
+                                            uint8_t** verticesToc, uint64_t** verticesData, uint64_t** histogram,
+                                            shb_marker_graph_result* result)
+{
+    return guarded([&] {
+        SHB_REQUIRE(c && params && (readGraphEdges || edgeCount == 0) && compressedToc && (compressedData || alignmentCount == 0) &&
+                    vertexTable && verticesToc && verticesData && histogram, SHB_ERR_INVALID, "Null argument.");
+        SHB_REQUIRE(readFlags || (c->haveMarkers && c->readCountTotal == 0), SHB_ERR_INVALID, "Null argument.");
+        createMarkerGraphVertices(c, *params, static_cast<const uint32_t*>(readGraphEdges), edgeCount, compressedToc, compressedData,
+                                  alignmentCount, readFlags, vertexTable, verticesToc, verticesData, histogram, result);
+    });
+}
+
+shb_status shb_find_marker_graph_reverse_complement_vertices(shb_context* c, const uint8_t* vertexTable, const uint8_t* verticesToc,
+                                                             const uint64_t* verticesData, uint64_t vertexCount, uint64_t** rcVertex)
+{
+    return guarded([&] {
+        SHB_REQUIRE(c && verticesToc && rcVertex && ((vertexTable && verticesData) || vertexCount == 0), SHB_ERR_INVALID, "Null argument.");
+        findMarkerGraphReverseComplementVertices(c, vertexTable, verticesToc, verticesData, vertexCount, rcVertex);
+    });
+}
+
+int shb_peak_finder_cutoff(const uint64_t* histogram, uint64_t n, double minAreaFraction, uint64_t startIndex, uint64_t* cutoff,
+                           double* observedAreaFraction)
+{
+    uint64_t x = 0;
+    double observed = 0;
+    const bool threw = peakFinderCutoff(histogram, n, minAreaFraction, startIndex, &x, &observed);
+    if(cutoff) *cutoff = x;
+    if(observedAreaFraction) *observedAreaFraction = observed;
+    return threw ? 1 : 0;
 }
 
 shb_status shb_test_radix_sort(shb_context* c, uint64_t* keys, uint32_t* values, uint64_t n,
