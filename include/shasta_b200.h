@@ -203,6 +203,9 @@ typedef struct {
     int32_t  maxMarkerFrequency;     /* method 0 only; ignored */
     int32_t  minAlignedMarkerCount;
     double   minAlignedFraction;
+    /* Scores of methods 1 and 3 (method 4 always scores 6/-1/-1). The DP runs in int32 with sentinels: a call is
+       refused with SHB_ERR_INVALID unless max(|match|, |mismatch|, |gap|) * (2 * L + 16384) < 2^28, L = the markers
+       of the longest read the call aligns (6/-1/-1: L up to 22.3 M). gapScore must not be positive. */
     int32_t  matchScore;
     int32_t  mismatchScore;
     int32_t  gapScore;

@@ -182,6 +182,7 @@ struct AlignCache {
     DeviceBuffer<uint32_t> sortedKmer, sortedOrdinal;
     uint64_t sortedGeneration = ~0ull;
     uint64_t lengthCheckGeneration = ~0ull;
+    uint64_t longestRead = 0;           // markers of the longest oriented read, for lengthCheckGeneration
     // workers and the device-side result accumulation: kept across calls so that a steady-state call does not allocate
     // or free device memory
     std::vector<std::unique_ptr<AlignWorker>> workers;
@@ -801,6 +802,52 @@ void computeAlignments(shb_context* c, const void* candidatesHost, uint64_t n, c
     }
 
     AlignCache& ac = *call.ac;
+    if(ac.lengthCheckGeneration != c->markerGeneration) {       // the traceback packs a run length above a 28-bit ordinal
+        uint64_t longest = 0;                                   // (the reference's Uint24 positions cap a read at 2^24 markers anyway)
+        for(size_t r = 0; r + 1 < c->tocHost.size(); r++) {
+            SHB_REQUIRE(c->tocHost[r + 1] - c->tocHost[r] < (1ull << kRunLengthShift), SHB_ERR_INVALID, "A read has 2^28 or more markers.");
+            longest = std::max<uint64_t>(longest, c->tocHost[r + 1] - c->tocHost[r]);
+        }
+        ac.longestRead = longest;
+        ac.lengthCheckGeneration = c->markerGeneration;
+    }
+    // Methods 1 and 3 use the configured scores; Align4 hard-codes 6/-1/-1 (src/Align4.hpp:159-161: never overwritten).
+    call.scores = call.method4 ? DpScores{6, -1, -1} : DpScores{o.matchScore, o.mismatchScore, o.gapScore};
+    // Score range of the DP kernels. They run in int32 with sentinels instead of "have" flags: kNegInf = -2^29 starts every
+    // cell outside the matrix, the two barrier offsets of the wavefront kernels enter with the gap score kGapBarrier = -2^28,
+    // and the end cell starts at -2^30. With M = max(|match|, |mismatch|, |gap|), L = longest read and W = kMaxBandWidth,
+    // their results equal exact arithmetic when M * (2L + W) < 2^28:
+    //  - every in-band cell of the matrix lies on a diagonal that starts at a boundary cell (score 0) inside the band, so its
+    //    exact score R satisfies |R| <= min(i, j) * M <= L * M, and every value in column i is at most i * M above anything
+    //    that does not enter through a barrier;
+    //  - an in-matrix cell only reads in-matrix cells and barriers (cells above the matrix feed only the row j = 0, which is
+    //    reset to 0; cells below it feed nothing), and every barrier value is kNegInf plus the drift of at most L + 31
+    //    columns (lanes start up to 31 columns early), or some earlier value plus kGapBarrier plus drift. Both are at most
+    //    L * M - 2^28 < -L * M <= R: a barrier never wins, nor ties, against a real score, and so never changes a trace code;
+    //  - the best end score is at least -L * M > -2^30, so it is always recorded;
+    //  - values stay within [-2^29 - (L + 64) * M - 2^28, (L + 2) * M], and the scan kernel's A - e * gap (e < W) within
+    //    (L + W + 1) * M of zero: nothing wraps.
+    // Under 6/-1/-1 (the defaults, and Align4 always) this admits reads of up to 22.3 M markers, more than the reference's
+    // 2^24-marker positions can hold; the 2^28-marker limit above alone would let a read exceed the sentinels.
+    // L is the longest read in the context (cached above); only when that fails are the reads of this call's candidates
+    // scanned, so that a context holding one very long read can still align the others.
+    {
+        const uint64_t M = uint64_t(std::max({std::abs(int64_t(call.scores.match)), std::abs(int64_t(call.scores.mismatch)),
+                                              std::abs(int64_t(call.scores.gap))}));
+        const auto fits = [M](uint64_t L) { return M * (2 * L + kMaxBandWidth) < (1ull << 28); };
+        if(!fits(ac.longestRead)) {
+            uint64_t longest = 0;
+            for(uint64_t i = 0; i < n; i++) {
+                for(int k = 0; k < 2; k++) {
+                    const uint64_t o = 2ull * call.cand[3 * i + k];
+                    longest = std::max<uint64_t>(longest, c->tocHost[o + 1] - c->tocHost[o]);
+                }
+            }
+            SHB_REQUIRE(fits(longest), SHB_ERR_INVALID,
+                        "Align scores too large for the reads: max(|matchScore|, |mismatchScore|, |gapScore|) * "
+                        "(2 * longest read in markers + 16384) must be below 2^28.");
+        }
+    }
     if(call.method4) {
         SHB_REQUIRE(o.align4DeltaX >= 1 && o.align4DeltaY >= 1 && o.align4DeltaX < (1ull << 31) && o.align4DeltaY < (1ull << 31),
                     SHB_ERR_INVALID, "Invalid Align.align4.deltaX / deltaY.");
@@ -808,17 +855,9 @@ void computeAlignments(shb_context* c, const void* candidatesHost, uint64_t n, c
     } else if(o.alignMethod == 3) {
         buildDownsampled(c, o.k, o.downsamplingFactor);
     }
-    if(ac.lengthCheckGeneration != c->markerGeneration) {       // the traceback packs a run length above a 28-bit ordinal
-        for(size_t r = 0; r + 1 < c->tocHost.size(); r++) {     // (the reference's Uint24 positions cap a read at 2^24 markers anyway)
-            SHB_REQUIRE(c->tocHost[r + 1] - c->tocHost[r] < (1ull << kRunLengthShift), SHB_ERR_INVALID, "A read has 2^28 or more markers.");
-        }
-        ac.lengthCheckGeneration = c->markerGeneration;
-    }
     const uint32_t maxStage2Width = uint32_t(std::max(0, o.maxBand)) + 3 + 64;     // W <= maxBand + 1, two barriers, padded to 64
     SHB_REQUIRE(maxStage2Width <= kMaxBandWidth, SHB_ERR_INVALID, "Align.maxBand too large for this implementation (limit 16317).");
 
-    // Methods 1 and 3 use the configured scores; Align4 hard-codes 6/-1/-1 (src/Align4.hpp:159-161: never overwritten).
-    call.scores = call.method4 ? DpScores{6, -1, -1} : DpScores{o.matchScore, o.mismatchScore, o.gapScore};
     call.fo.minAlignedMarkerCount = uint64_t(o.minAlignedMarkerCount); call.fo.maxSkip = uint64_t(o.maxSkip);
     call.fo.maxDrift = uint64_t(o.maxDrift); call.fo.maxTrim = uint64_t(o.maxTrim);
     call.fo.minAlignedFraction = o.minAlignedFraction;

@@ -9,7 +9,8 @@ oracle's under B.set_dp_policy(N): records, compressed toc and bytes, and the de
 Most cases run on reads cut from a genome of eight k-mer ids, where ties are everywhere. They cover every kernel whose
 output depends on the policy: method 3 stage 2 on the 8-lane group classes, the whole-warp classes and the scan kernel;
 method 3 stage 1 on the forward kernel (groups of 8, 16 and 32 lanes) and on the traced path; method 1 up to the scan
-kernel; method 4; the single-pair entry point with methods 1, 3 and 4; four score sets; the k = 10 synthetic reads; and
+kernel; method 4; the single-pair entry point with methods 1, 3 and 4; eight score sets, from the shipped 6/-1/-1 to 0/0/0,
+2/5/-1 (a mismatch above a match), 6/0/0 and 1/-1000/-1; the k = 10 synthetic reads; and
 pairs built so that the best end score is 0 and is reached both in the last row and at the boundary cell (nx, 0), where
 the last-maximum end-cell rule must pick (nx, 0) and store nothing.
 
@@ -38,7 +39,11 @@ from shasta_b200 import synth  # noqa: E402
 K = AL.K
 DEFAULT_POLICY = 7
 POLICY_DIR = os.path.join(ROOT, "shasta_b200", "lib", "dp_policy")
-SCORES = {"6_1_1": (6, -1, -1), "6_1_3": (6, -1, -3), "6_1_0": (6, -1, 0), "3_2_1": (3, -2, -1)}
+# The shipped 6/-1/-1 and variants, then unusual but legal sets: every path ties (0/0/0), a mismatch scoring above a match
+# (2/5/-1: stage-1 paths of diagonal steps with no matching k-mer, whose band wraps around and is skipped), free gaps and
+# mismatches (6/0/0), and a mismatch far costlier than a gap (1/-1000/-1).
+SCORES = {"6_1_1": (6, -1, -1), "6_1_3": (6, -1, -3), "6_1_0": (6, -1, 0), "3_2_1": (3, -2, -1),
+          "0_0_0": (0, 0, 0), "2_5_1": (2, 5, -1), "6_0_0": (6, 0, 0), "1_1000_1": (1, -1000, -1)}
 FORWARD_GROUPS = ((128, 8), (256, 16), (512, 32))      # dpForwardClassAt: rows held by groups of 8, 16, 32 lanes
 SCAN_MIN_WIDTH = 1023                                   # bands of more offsets run on the scan kernel (dpClassAt)
 
@@ -379,6 +384,48 @@ def test_each_policy_bit_changes_the_stored_output():
             if other < policy:
                 continue
             assert any(stored[policy][name] != stored[other][name] for name in stored[policy]), (policy, other)
+
+
+INT32_MAX, INT32_MIN = (1 << 31) - 1, -(1 << 31)
+
+
+def wrap32(x):
+    return (x - INT32_MIN) % (1 << 32) + INT32_MIN
+
+
+def stage1_outcome(a, b, opts, sc):
+    """What method 3's stage 1 leaves for stage 2 under the oracle's current policy: 'none' (no diagonal step), 'no_match'
+    (diagonal steps, none on equal k-mers) or 'band'."""
+    (da, _), (db, _) = downsampled(a, opts["downsamplingFactor"]), downsampled(b, opts["downsamplingFactor"])
+    _, path = B.overlap_align(da, db, *sc)
+    if not len(path):
+        return "none"
+    return "band" if (da[path[:, 0]] == db[path[:, 1]]).any() else "no_match"
+
+
+def test_stage1_without_a_matching_step_is_reached():
+    # 2/5/-1 prefers mismatches: stage-1 paths with diagonal steps and no matching k-mer (kPairNoMatchingStep on the forward
+    # kernel, INT32_MAX / INT32_MIN offsets on the traced path). setStage2Band widens them by bandExtend in 32-bit
+    # wrap-around arithmetic: the band's width wraps to 2 * bandExtend <= maxBand, but bandMin > bandMax, so the candidate
+    # is skipped (the reference's SeqAn throw); the oracle stores nothing for it.
+    case = {c.name: c for c in cases()}["m3_ties_s2_5_1"]
+    opts, sc = case.opts, SCORES["2_5_1"]
+    band_min, band_max = wrap32(INT32_MAX - opts["bandExtend"]), wrap32(INT32_MIN + opts["bandExtend"])
+    assert wrap32(band_max - band_min) <= opts["maxBand"] and band_min > band_max
+    d, cand = tie_set()
+    reached = set()
+    for c in cand:
+        a, b = candidate_rows(d, c)
+        if stage1_outcome(a, b, opts, sc) == "no_match":
+            reached.add(forward_lanes(len(downsampled(b, opts["downsamplingFactor"])[0])) is not None)
+            status, ords, _ = B.oracle_align_pair(a, b, oracle_options(opts))
+            assert status == 1 and len(ords) == 0
+    assert reached == {True, False}         # on the forward kernel and on the traced path
+    # ... and the candidates are not stored: none of them appears in the oracle's output of the case.
+    stored = _stored(*oracle_outputs(DEFAULT_POLICY)[case.name])
+    keys = {tuple(int(x) for x in c) for c in cand
+            if stage1_outcome(*candidate_rows(d, c), opts, sc) == "no_match"}
+    assert keys and not keys & set(stored)
 
 
 def dp_scores(a, b, match, mismatch, gap):
