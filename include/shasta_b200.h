@@ -338,7 +338,10 @@ shb_status shb_palindromic_read_alignment(shb_context* ctx, uint64_t readId, con
  *   keep             : receives uint8[n] (1 = used in the read graph).
  *   edges            : receives edgeCount 16-byte ReadGraphEdge records (src/ReadGraph.hpp:37-57) = Data/ReadGraphEdges payload.
  *   connectivityToc  : receives uint32[2*readCount+1]; connectivityData: uint32[2*edgeCount] = Data/ReadGraphConnectivity
- *                      (.toc/.data payload, VectorOfVectors<uint32_t,uint32_t>): per oriented read its edge indices, increasing.
+ *                      (.toc/.data payload, VectorOfVectors<uint32_t,uint32_t>): per oriented read its edge indices, DECREASING
+ *                      (the reference's VectorOfVectors::store fills each row from its end).
+ * A kept alignment whose edge or reverse-complement edge is not ordered (readIds[0] > readIds[1], or a read aligned to
+ * itself: the reference's SHASTA_ASSERT) returns SHB_ERR_INVALID naming the alignment; alignmentData is then left unchanged.
  * Free the four arrays with shb_free. (creationMethod 2: shb_create_read_graph2 below.)
  */
 shb_status shb_create_read_graph(shb_context* ctx, void* alignmentData, uint64_t alignmentCount, uint64_t readCount,

@@ -56,6 +56,16 @@ def have_ref():
     return os.path.exists(REF_SO)
 
 
+def have_ref_readgraph():
+    """The reference build is present AND has the read graph glue (ref_glue/ref_readgraph.cpp's table and read graph entry
+    points). A prebuilt oracle/_ref from before that glue lacks them: the tests then use the recorded outputs instead."""
+    if not have_ref():
+        return False
+    lib = ref_lib()
+    return all(hasattr(lib, name) for name in ("ref_compute_alignment_table", "ref_compute_candidate_table",
+                                               "ref_create_read_graph", "ref_create_read_graph2"))
+
+
 def ref_lib():
     global _ref
     if _ref is None:
@@ -445,43 +455,122 @@ def oracle_compute_candidate_table(candidates, read_count):
     return toc, table[:4 * len(cand)].copy()
 
 
-def oracle_create_read_graph(records, read_count, max_alignment_count):
-    """Assembler::createReadGraph, creationMethod 0 (src/AssemblerReadGraph.cpp:35-175). records uint32[n,16] is NOT modified.
-    Returns (records with isInReadGraph set, keep uint8[n], edges uint32[E,4], connectivityToc uint32[2R+1], connectivityData uint32[2E])."""
-    lib = _olib()
+class UnorderedReadGraphEdge(ValueError):
+    """A kept alignment gives a read graph edge, or a reverse-complement edge, whose oriented reads are not in increasing
+    order: the SHASTA_ASSERT of src/AssemblerReadGraph.cpp:134,140."""
+
+
+def _read_graph_buffers(records, read_count):
     rec = np.ascontiguousarray(records, np.uint32).reshape(-1, 16).copy()
     n = len(rec)
-    keep = np.zeros(n + 1, np.uint8)
-    edges = np.zeros((2 * n + 1, 4), np.uint32)
-    toc = np.zeros(2 * read_count + 1, np.uint32)
-    data = np.zeros(4 * n + 1, np.uint32)
-    lib.orc_create_read_graph.restype = C.c_uint64
-    lib.orc_create_read_graph.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-    e = lib.orc_create_read_graph(rec.ctypes.data, n, read_count, int(max_alignment_count), keep.ctypes.data, edges.ctypes.data,
-                                  toc.ctypes.data, data.ctypes.data)
+    return rec, np.zeros(n + 1, np.uint8), np.zeros((2 * n + 1, 4), np.uint32), np.zeros(2 * read_count + 1, np.uint32), \
+        np.zeros(4 * n + 1, np.uint32)
+
+
+def _criteria(crit):
+    return dict(minAlignedFraction=float(crit[:1].view(np.float64)[0]), minAlignedMarkerCount=int(crit[1]), maxDrift=int(crit[2]),
+                maxSkip=int(crit[3]), maxTrim=int(crit[4]))
+
+
+def oracle_create_read_graph(records, read_count, max_alignment_count):
+    """Assembler::createReadGraph, creationMethod 0 (src/AssemblerReadGraph.cpp:35-175). records uint32[n,16] is NOT modified.
+    Returns (records with isInReadGraph set, keep uint8[n], edges uint32[E,4], connectivityToc uint32[2R+1], connectivityData uint32[2E]);
+    each connectivity row lists its edges in decreasing edge index, as the reference's VectorOfVectors::store leaves them.
+    Raises UnorderedReadGraphEdge where the reference's assertion fails."""
+    lib = _olib()
+    rec, keep, edges, toc, data = _read_graph_buffers(records, read_count)
+    n = len(rec)
+    e = C.c_uint64()
+    lib.orc_create_read_graph.restype = C.c_int
+    lib.orc_create_read_graph.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p]
+    if lib.orc_create_read_graph(rec.ctypes.data, n, read_count, int(max_alignment_count), keep.ctypes.data, edges.ctypes.data,
+                                 C.byref(e), toc.ctypes.data, data.ctypes.data):
+        raise UnorderedReadGraphEdge("a kept alignment gives an unordered read graph edge")
+    e = e.value
     return rec, keep[:n].copy(), edges[:e].copy(), toc, data[:2 * e].copy()
 
 
 def oracle_create_read_graph2(records, read_count, max_alignment_count, percentiles):
     """Assembler::createReadGraph2, creationMethod 2 (src/AssemblerReadGraph2.cpp:69-248). percentiles = (markerCount,
-    alignedFraction, maxSkip, maxDrift, maxTrim). Returns (criteria dict, records, keep, edges, connectivityToc, connectivityData)."""
+    alignedFraction, maxSkip, maxDrift, maxTrim). Returns (criteria dict, records, keep, edges, connectivityToc, connectivityData),
+    the last five as in oracle_create_read_graph."""
     lib = _olib()
-    rec = np.ascontiguousarray(records, np.uint32).reshape(-1, 16).copy()
+    rec, keep, edges, toc, data = _read_graph_buffers(records, read_count)
     n = len(rec)
-    keep = np.zeros(n + 1, np.uint8)
-    edges = np.zeros((2 * n + 1, 4), np.uint32)
-    toc = np.zeros(2 * read_count + 1, np.uint32)
-    data = np.zeros(4 * n + 1, np.uint32)
     pc = np.array(percentiles, np.float64)
     crit = np.zeros(5, np.uint64)
-    lib.orc_create_read_graph2.restype = C.c_uint64
+    e = C.c_uint64()
+    lib.orc_create_read_graph2.restype = C.c_int
     lib.orc_create_read_graph2.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                           C.c_void_p, C.c_void_p]
-    e = lib.orc_create_read_graph2(rec.ctypes.data, n, read_count, int(max_alignment_count), pc.ctypes.data, crit.ctypes.data,
-                                   keep.ctypes.data, edges.ctypes.data, toc.ctypes.data, data.ctypes.data)
-    criteria = dict(minAlignedFraction=float(crit[:1].view(np.float64)[0]), minAlignedMarkerCount=int(crit[1]), maxDrift=int(crit[2]),
-                    maxSkip=int(crit[3]), maxTrim=int(crit[4]))
-    return criteria, rec, keep[:n].copy(), edges[:e].copy(), toc, data[:2 * e].copy()
+                                           C.c_void_p, C.c_void_p, C.c_void_p]
+    if lib.orc_create_read_graph2(rec.ctypes.data, n, read_count, int(max_alignment_count), pc.ctypes.data, crit.ctypes.data,
+                                  keep.ctypes.data, edges.ctypes.data, C.byref(e), toc.ctypes.data, data.ctypes.data):
+        raise UnorderedReadGraphEdge("a kept alignment gives an unordered read graph edge")
+    e = e.value
+    return _criteria(crit), rec, keep[:n].copy(), edges[:e].copy(), toc, data[:2 * e].copy()
+
+
+def ref_create_read_graph(records, read_count, max_alignment_count):
+    """The reference's createReadGraph and createReadGraphUsingSelectedAlignments over its own containers
+    (oracle/ref_glue/ref_readgraph.cpp). Same arguments, returns and refusal as oracle_create_read_graph."""
+    lib = _rlib()
+    rec, keep, edges, toc, data = _read_graph_buffers(records, read_count)
+    n = len(rec)
+    e = C.c_uint64()
+    lib.ref_create_read_graph.restype = C.c_int
+    lib.ref_create_read_graph.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p]
+    if lib.ref_create_read_graph(rec.ctypes.data, n, read_count, int(max_alignment_count), keep.ctypes.data, edges.ctypes.data,
+                                 C.byref(e), toc.ctypes.data, data.ctypes.data):
+        raise UnorderedReadGraphEdge("the reference refused the read graph")
+    e = e.value
+    return rec, keep[:n].copy(), edges[:e].copy(), toc, data[:2 * e].copy()
+
+
+def ref_create_read_graph2(records, read_count, max_alignment_count, percentiles):
+    """The reference's createReadGraph2 (Histogram2 criteria, then the selection of createReadGraph) over its own containers.
+    Same arguments, returns and refusal as oracle_create_read_graph2."""
+    lib = _rlib()
+    rec, keep, edges, toc, data = _read_graph_buffers(records, read_count)
+    n = len(rec)
+    pc = np.array(percentiles, np.float64)
+    crit = np.zeros(5, np.uint64)
+    e = C.c_uint64()
+    lib.ref_create_read_graph2.restype = C.c_int
+    lib.ref_create_read_graph2.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_void_p]
+    if lib.ref_create_read_graph2(rec.ctypes.data, n, read_count, int(max_alignment_count), pc.ctypes.data, crit.ctypes.data,
+                                  keep.ctypes.data, edges.ctypes.data, C.byref(e), toc.ctypes.data, data.ctypes.data):
+        raise UnorderedReadGraphEdge("the reference refused the read graph")
+    e = e.value
+    return _criteria(crit), rec, keep[:n].copy(), edges[:e].copy(), toc, data[:2 * e].copy()
+
+
+def ref_compute_alignment_table(records, read_count):
+    """The reference's computeAlignmentTable over its own VectorOfVectors. Returns (toc uint32[2R+1], table uint32[4n])."""
+    lib = _rlib()
+    rec = np.ascontiguousarray(records, np.uint32).reshape(-1, 16)
+    toc = np.zeros(2 * read_count + 1, np.uint32)
+    table = np.zeros(4 * len(rec) + 1, np.uint32)
+    lib.ref_compute_alignment_table.restype = C.c_int
+    lib.ref_compute_alignment_table.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]
+    if lib.ref_compute_alignment_table(rec.ctypes.data, len(rec), read_count, toc.ctypes.data, table.ctypes.data):
+        raise RuntimeError("reference computeAlignmentTable failed")
+    return toc, table[:4 * len(rec)].copy()
+
+
+def ref_compute_candidate_table(candidates, read_count):
+    """The reference's computeCandidateTable over its own VectorOfVectors. Returns (toc uint64[2R+1], table uint64[4n])."""
+    lib = _rlib()
+    cand = np.ascontiguousarray(candidates, np.uint32).reshape(-1, 3)
+    toc = np.zeros(2 * read_count + 1, np.uint64)
+    table = np.zeros(4 * len(cand) + 1, np.uint64)
+    lib.ref_compute_candidate_table.restype = C.c_int
+    lib.ref_compute_candidate_table.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]
+    if lib.ref_compute_candidate_table(cand.ctypes.data, len(cand), read_count, toc.ctypes.data, table.ctypes.data):
+        raise RuntimeError("reference computeCandidateTable failed")
+    return toc, table[:4 * len(cand)].copy()
 
 
 def oracle_histogram2_threshold(x, start, stop, bin_count, fraction):

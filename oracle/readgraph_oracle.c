@@ -1,7 +1,8 @@
 /* TEST INFRASTRUCTURE (oracle): CPU restatement of Assembler::createReadGraph, ReadGraph.creationMethod 0
- * (src/AssemblerReadGraph.cpp:35-175). Only tests/ may call it. Parity status: a restatement only (the member needs the
- * whole Assembler, which is unbuildable here); it follows the reference's control flow with qsort in place of
- * std::nth_element — the SET nth_element leaves in the first maxAlignmentCount places is the same. */
+ * (src/AssemblerReadGraph.cpp:35-175). Only tests/ may call it. Parity status: a restatement, pinned against the reference's
+ * own code by tests/test_oracle_readgraph.py (oracle/ref_glue/ref_readgraph.cpp follows the member over the reference's
+ * containers). It follows the reference's control flow with qsort in place of std::nth_element — the SET nth_element
+ * leaves in the first maxAlignmentCount places is the same. */
 #include <math.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -19,10 +20,13 @@ static int greaterFirst(const void* a, const void* b)
 }
 
 /* alignmentData: n 64-byte records (in/out: isInReadGraph). keep: uint8[n]. edges: room for 2n 16-byte records.
- * connToc: uint32[2*readCount+1], connData: uint32[4n]. Returns the number of edges. */
-static uint64_t createReadGraph(uint32_t* alignmentData, uint64_t n, uint64_t readCount, uint32_t maxAlignmentCount,
-                                const uint8_t* eligible /* null: every alignment */,
-                                uint8_t* keep, uint32_t* edges, uint32_t* connToc, uint32_t* connData)
+ * connToc: uint32[2*readCount+1], connData: uint32[4n]. *edgeCountOut: the number of edges. Returns 0, or 1 when a kept
+ * alignment gives an edge, or a reverse-complement edge, whose oriented reads are not in increasing order: the reference's
+ * SHASTA_ASSERT at src/AssemblerReadGraph.cpp:134,140 (readIds[0] > readIds[1], or a read aligned to itself). An alignment
+ * that is not kept is never looked at there, so it may be unordered. */
+static int createReadGraph(uint32_t* alignmentData, uint64_t n, uint64_t readCount, uint32_t maxAlignmentCount,
+                           const uint8_t* eligible /* null: every alignment */,
+                           uint8_t* keep, uint32_t* edges, uint64_t* edgeCountOut, uint32_t* connToc, uint32_t* connData)
 {
     memset(keep, 0, n);
     /* the rows (readId, 0) of the alignment table: every alignment of the read (src/AssemblerAlign.cpp:509-571) */
@@ -56,36 +60,41 @@ static uint64_t createReadGraph(uint32_t* alignmentData, uint64_t n, uint64_t re
     free(all); free(fill); free(count);
     /* createReadGraphUsingSelectedAlignments :95-144 */
     uint64_t edgeCount = 0;
+    *edgeCountOut = 0;
     for(uint64_t a = 0; a < n; a++) {
         uint32_t* rec = alignmentData + 16 * a;
         rec[15] = (rec[15] & ~1u) | keep[a];
         if(!keep[a]) continue;
         const uint32_t o0 = 2 * rec[0], o1 = 2 * rec[1] + ((rec[2] & 0xff) ? 0u : 1u);
+        if(!(o0 < o1 && (o0 ^ 1u) < (o1 ^ 1u))) return 1;
         for(uint32_t k = 0; k < 2; k++) {
             uint32_t* e = edges + 4 * edgeCount;
             e[0] = o0 ^ k; e[1] = o1 ^ k; e[2] = (uint32_t)a; e[3] = 0;
             edgeCount++;
         }
     }
-    /* connectivity :147-159 */
+    /* connectivity :147-159. MemoryMapped::VectorOfVectors::store fills a row from its end
+     * (src/MemoryMappedVectorOfVectors.hpp:384-387) and the edges are stored in increasing order, so every row lists its
+     * edges in DECREASING edge index. */
     const uint64_t rows = 2 * readCount;
     memset(connToc, 0, (rows + 1) * sizeof(uint32_t));
     for(uint64_t i = 0; i < edgeCount; i++) { connToc[edges[4 * i] + 1]++; connToc[edges[4 * i + 1] + 1]++; }
     for(uint64_t r = 0; r < rows; r++) connToc[r + 1] += connToc[r];
-    uint32_t* at = (uint32_t*)malloc((rows + 1) * sizeof(uint32_t));
-    memcpy(at, connToc, (rows + 1) * sizeof(uint32_t));
+    uint32_t* end = (uint32_t*)malloc((rows + 1) * sizeof(uint32_t));
+    memcpy(end, connToc + 1, rows * sizeof(uint32_t));
     for(uint64_t i = 0; i < edgeCount; i++) {
-        connData[at[edges[4 * i]]++] = (uint32_t)i;
-        connData[at[edges[4 * i + 1]]++] = (uint32_t)i;
+        connData[--end[edges[4 * i]]] = (uint32_t)i;
+        connData[--end[edges[4 * i + 1]]] = (uint32_t)i;
     }
-    free(at);
-    return edgeCount;
+    free(end);
+    *edgeCountOut = edgeCount;
+    return 0;
 }
 
-uint64_t orc_create_read_graph(uint32_t* alignmentData, uint64_t n, uint64_t readCount, uint32_t maxAlignmentCount,
-                               uint8_t* keep, uint32_t* edges, uint32_t* connToc, uint32_t* connData)
+int orc_create_read_graph(uint32_t* alignmentData, uint64_t n, uint64_t readCount, uint32_t maxAlignmentCount,
+                          uint8_t* keep, uint32_t* edges, uint64_t* edgeCount, uint32_t* connToc, uint32_t* connData)
 {
-    return createReadGraph(alignmentData, n, readCount, maxAlignmentCount, NULL, keep, edges, connToc, connData);
+    return createReadGraph(alignmentData, n, readCount, maxAlignmentCount, NULL, keep, edges, edgeCount, connToc, connData);
 }
 
 /* shasta::Histogram2 with dynamicBounds = true (src/Histogram.cpp:14-140), restated with the effect of its update():
@@ -151,9 +160,9 @@ static Indicators indicators(const uint32_t* rec)
 
 /* createReadGraph2, src/AssemblerReadGraph2.cpp:99-248. percentiles: markerCount, alignedFraction, maxSkip, maxDrift, maxTrim.
  * criteria: double minAlignedFraction, then uint64 minAlignedMarkerCount, maxDrift, maxSkip, maxTrim (as 5 x 8 bytes). */
-uint64_t orc_create_read_graph2(uint32_t* alignmentData, uint64_t n, uint64_t readCount, uint32_t maxAlignmentCount,
-                                const double* percentiles, void* criteria,
-                                uint8_t* keep, uint32_t* edges, uint32_t* connToc, uint32_t* connData)
+int orc_create_read_graph2(uint32_t* alignmentData, uint64_t n, uint64_t readCount, uint32_t maxAlignmentCount,
+                           const double* percentiles, void* criteria,
+                           uint8_t* keep, uint32_t* edges, uint64_t* edgeCount, uint32_t* connToc, uint32_t* connData)
 {
     Hist af, mc, dr, sk, tr;
     histInit(&af, 0, 1, 100); histInit(&mc, 0, 3000, 300); histInit(&dr, 0, 100, 100); histInit(&sk, 0, 100, 100); histInit(&tr, 0, 100, 100);
@@ -177,7 +186,7 @@ uint64_t orc_create_read_graph2(uint32_t* alignmentData, uint64_t n, uint64_t re
         eligible[i] = !(a.minAlignedFraction < minAlignedFraction) && !(a.markerCount < minAlignedMarkerCount) &&
                       !(a.maxDrift > maxDrift) && !(a.maxSkip > maxSkip) && !(a.trim > maxTrim);
     }
-    const uint64_t e = createReadGraph(alignmentData, n, readCount, maxAlignmentCount, eligible, keep, edges, connToc, connData);
+    const int status = createReadGraph(alignmentData, n, readCount, maxAlignmentCount, eligible, keep, edges, edgeCount, connToc, connData);
     free(eligible);
-    return e;
+    return status;
 }

@@ -440,7 +440,9 @@ def compute_alignment_table(ctx: Context, records, read_count):
 def create_read_graph(ctx: Context, records, read_count, max_alignment_count):
     """Assembler::createReadGraph, ReadGraph.creationMethod 0 (shb_create_read_graph). records uint32[n,16] must be a writable,
     C-contiguous array: AlignmentInfo::isInReadGraph is updated in place.
-    Returns (keep uint8[n], edges uint32[E,4] = 16-byte ReadGraphEdge records, connectivityToc uint32[2R+1], connectivityData uint32[2E])."""
+    Returns (keep uint8[n], edges uint32[E,4] = 16-byte ReadGraphEdge records, connectivityToc uint32[2R+1], connectivityData uint32[2E]);
+    each connectivity row lists its edges in decreasing edge index, the reference's order. A kept alignment whose edge is not
+    ordered (readIds[0] > readIds[1], or a read aligned to itself) raises ShastaB200Error (SHB_ERR_INVALID), records untouched."""
     assert records.dtype == np.uint32 and records.flags["C_CONTIGUOUS"] and records.flags["WRITEABLE"]
     rec = records.reshape(-1, 16)
     keep, edges, toc, data = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
@@ -465,7 +467,7 @@ class ReadGraph2Criteria(C.Structure):
 def create_read_graph2(ctx: Context, records, read_count, max_alignment_count, marker_count_percentile, aligned_fraction_percentile,
                        max_skip_percentile, max_drift_percentile, max_trim_percentile):
     """Assembler::createReadGraph2, ReadGraph.creationMethod 2 (shb_create_read_graph2). records as in create_read_graph.
-    Returns (criteria dict, keep, edges, connectivityToc, connectivityData)."""
+    Returns (criteria dict, keep, edges, connectivityToc, connectivityData), and refuses what create_read_graph refuses."""
     assert records.dtype == np.uint32 and records.flags["C_CONTIGUOUS"] and records.flags["WRITEABLE"]
     rec = records.reshape(-1, 16)
     keep, edges, toc, data = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()

@@ -6,8 +6,12 @@
 //     DESCENDING alignmentId order and stably sorted by (readId ascending, markerCount descending): an item's rank inside
 //     its read is its distance from the read's first item;
 //   * an alignment is kept when it is among the best of EITHER of its reads (:77-85); kept alignments get
-//     AlignmentInfo::isInReadGraph (:103) and two edges each, in alignmentId order (:110-140);
-//   * ReadGraphConnectivity: for every oriented read the indices of its edges in increasing order (:147-159).
+//     AlignmentInfo::isInReadGraph (:103) and two edges each, in alignmentId order (:110-140). A kept alignment whose edge
+//     or reverse-complement edge is not ordered (readIds[0] > readIds[1], or a read aligned to itself) is refused, where
+//     the reference stops on SHASTA_ASSERT (:134, :140);
+//   * ReadGraphConnectivity: for every oriented read the indices of its edges in DECREASING order (:147-159): the
+//     reference stores the edges in increasing order and MemoryMapped::VectorOfVectors::store fills each row from its end
+//     (src/MemoryMappedVectorOfVectors.hpp:384-387).
 // Assembler::createReadGraph2, ReadGraph.creationMethod 2 (src/AssemblerReadGraph2.cpp:182-248; what Nanopore-May2022.conf and
 // Nanopore-UL-May2022.conf select): the same selection over the alignments that pass five thresholds, which are read off
 // histograms of the alignments' quality indicators at given percentiles (setReadGraph2Criteria, :99-179). The histograms are
@@ -53,9 +57,13 @@ __global__ void readGraphKeepKernel(const uint64_t* __restrict__ sortedKeys, con
 }
 
 // 16-byte ReadGraphEdge (src/ReadGraph.hpp:37-57): orientedReadIds[2], alignmentId:62 | crossesStrands:1 | hasInconsistentAlignment:1.
+// The (row, edge) entries are written in DECREASING edge order, so the stable sort on the row alone leaves every row in
+// decreasing edge order, the reference's. That costs nothing beyond the index arithmetic; sorting on (row, ~edge) instead
+// would add radix passes over the edge bits. The two entries of one edge have different rows (the edge is ordered), so
+// their relative order does not matter.
 __global__ void readGraphEdgesKernel(const uint32_t* __restrict__ records, uint32_t n, const uint32_t* __restrict__ keep,
-                                     const uint32_t* __restrict__ keepIndex, uint32_t* __restrict__ edges, uint64_t* __restrict__ rowKeys,
-                                     uint32_t* __restrict__ rowVals)
+                                     const uint32_t* __restrict__ keepIndex, uint32_t entries, uint32_t* __restrict__ edges,
+                                     uint64_t* __restrict__ rowKeys, uint32_t* __restrict__ rowVals)
 {
     const uint32_t a = blockIdx.x * blockDim.x + threadIdx.x;
     if(a >= n || !keep[a]) return;
@@ -67,8 +75,9 @@ __global__ void readGraphEdgesKernel(const uint32_t* __restrict__ records, uint3
     for(uint32_t k = 0; k < 2; k++) {                   // the edge and its reverse complement
         uint32_t* w = edges + 4ull * (e + k);
         w[0] = o0 ^ k; w[1] = o1 ^ k; w[2] = a; w[3] = 0u;      // alignmentId < 2^32: the flags in the top two bits stay 0
-        rowKeys[2ull * (e + k)] = uint64_t(o0 ^ k) << 32;      rowVals[2ull * (e + k)] = e + k;
-        rowKeys[2ull * (e + k) + 1] = uint64_t(o1 ^ k) << 32;  rowVals[2ull * (e + k) + 1] = e + k;
+        const uint64_t slot = uint64_t(entries) - 2u * (e + k + 1u);     // edge e + k from the back
+        rowKeys[slot] = uint64_t(o0 ^ k) << 32;      rowVals[slot] = e + k;
+        rowKeys[slot + 1] = uint64_t(o1 ^ k) << 32;  rowVals[slot + 1] = e + k;
     }
 }
 
@@ -221,7 +230,7 @@ void createReadGraph(shb_context* c, void* alignmentData, uint64_t n, uint64_t r
         dEdges.reserve(4ull * edgeCount); dToc.reserve(uint64_t(rows) + 1);
         // the item buffers are free again: reuse them for the (row, edge) entries
         SHB_LAUNCH(readGraphEdgesKernel, ceilDiv(n, 256), 256, 0, st, (const uint32_t*)dRec.get(), uint32_t(n), (const uint32_t*)keep.get(),
-                   (const uint32_t*)keepIndex.get(), dEdges.get(), keysA.get(), valsA.get());
+                   (const uint32_t*)keepIndex.get(), entries, dEdges.get(), keysA.get(), valsA.get());
         uint32_t rowBits = 1;
         while((1ull << rowBits) < uint64_t(rows)) rowBits++;
         const int ranges[1][2] = {{32, 32 + int(rowBits)}};
@@ -236,6 +245,18 @@ void createReadGraph(shb_context* c, void* alignmentData, uint64_t n, uint64_t r
         SHB_CUDA(cudaMemcpyAsync(keepWords.data(), keep.get(), 4ull * n, cudaMemcpyDeviceToHost, st));
         SHB_CUDA(cudaStreamSynchronize(st));
         for(uint64_t i = 0; i < n; i++) keepHost[i] = uint8_t(keepWords[i]);
+    }
+    // src/AssemblerReadGraph.cpp:134,140: SHASTA_ASSERT(edge.orientedReadIds[0] < edge.orientedReadIds[1]) for every kept
+    // alignment, on the edge and on its reverse complement. Checked before isInReadGraph is written, so a refused call leaves
+    // the records as they were.
+    for(uint64_t i = 0; i < n; i++) {
+        if(!keepHost[i]) continue;
+        const uint32_t* r = rec + kAlignmentWords * i;
+        const uint32_t o0 = 2u * r[0], o1 = 2u * r[1] + ((r[2] & 0xffu) ? 0u : 1u);
+        SHB_REQUIRE(o0 < o1 && (o0 ^ 1u) < (o1 ^ 1u), SHB_ERR_INVALID,
+                    "Alignment " + std::to_string(i) + " (reads " + std::to_string(r[0]) + " and " + std::to_string(r[1]) +
+                    ((r[2] & 0xffu) ? ", same strand" : ", opposite strands") +
+                    ") is kept for the read graph but its oriented reads are not in increasing order.");
     }
     // AlignmentInfo::isInReadGraph (src/Alignment.hpp:194: bit 0 of the flag byte after maxDrift), src/AssemblerReadGraph.cpp:103.
     for(uint64_t i = 0; i < n; i++) {

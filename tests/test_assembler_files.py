@@ -212,6 +212,13 @@ def test_script_sequence_on_reference_data_dir(tmp_path, golden_dir, monkeypatch
     ctoc = np.asarray(A.mm_read_vector(prefix + "ReadGraphConnectivity.toc", np.uint32, object_size=4))
     cdata = np.asarray(A.mm_read_vector(prefix + "ReadGraphConnectivity.data", np.uint32, object_size=4))
     assert np.array_equal(edges, wedges) and np.array_equal(ctoc, wtoc) and np.array_equal(cdata, wdata)
+    if B.have_ref_readgraph():
+        # the reference's own createReadGraph on the same AlignmentData (oracle/ref_glue/ref_readgraph.cpp), and the
+        # connectivity files as the reference's MemoryMapped::Vector opens them
+        _, _, redges, rtoc, rdata = B.ref_create_read_graph(rec, 20, 3)
+        assert np.array_equal(edges, redges) and np.array_equal(ctoc, rtoc) and np.array_equal(cdata, rdata)
+        assert B.ref_open_vector(prefix + "ReadGraphConnectivity.toc", 4) == (len(rtoc), fnv(rtoc.tobytes()))
+        assert B.ref_open_vector(prefix + "ReadGraphConnectivity.data", 4) == (len(rdata), fnv(rdata.tobytes()))
     # ... and ReadGraph.creationMethod 2 (srcMain/main.cpp:731-739), the one the May2022 configurations select
     f = A.Assembler(largeDataFileNamePrefix=prefix)
     f.accessMarkers()
@@ -220,7 +227,13 @@ def test_script_sequence_on_reference_data_dir(tmp_path, golden_dir, monkeypatch
     crit2, wrec2, wkeep2, wedges2, wtoc2, wdata2 = B.oracle_create_read_graph2(rec, 20, 3, (0.015, 0.12, 0.12, 0.12, 0.015))
     assert kept2 == int(wkeep2.sum()) and f.readGraph2Criteria == crit2
     edges2 = np.asarray(A.mm_read_vector(prefix + "ReadGraphEdges", np.uint32, object_size=16)).reshape(-1, 4)
-    assert np.array_equal(edges2, wedges2)
+    ctoc2 = np.asarray(A.mm_read_vector(prefix + "ReadGraphConnectivity.toc", np.uint32, object_size=4))
+    cdata2 = np.asarray(A.mm_read_vector(prefix + "ReadGraphConnectivity.data", np.uint32, object_size=4))
+    assert np.array_equal(edges2, wedges2) and np.array_equal(ctoc2, wtoc2) and np.array_equal(cdata2, wdata2)
+    if B.have_ref_readgraph():
+        rcrit2, _, _, redges2, rtoc2, rdata2 = B.ref_create_read_graph2(rec, 20, 3, (0.015, 0.12, 0.12, 0.12, 0.015))
+        assert rcrit2 == crit2 and np.array_equal(edges2, redges2) and np.array_equal(ctoc2, rtoc2) and np.array_equal(cdata2, rdata2)
+        assert B.ref_open_vector(prefix + "ReadGraphConnectivity.data", 4) == (len(rdata2), fnv(rdata2.tobytes()))
     # srcMain/main.cpp:706: computeCandidateTable after the candidates are known
     b.computeCandidateTable()
     ct_toc = np.asarray(A.mm_read_vector(prefix + "CandidateTable.toc", np.uint64, object_size=8))
