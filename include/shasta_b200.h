@@ -363,6 +363,56 @@ shb_status shb_create_read_graph2(shb_context* ctx, void* alignmentData, uint64_
                                   shb_read_graph2_criteria* criteria, uint8_t** keep, void** edges, uint64_t* edgeCount,
                                   uint32_t** connectivityToc, uint32_t** connectivityData);
 
+// ---- flagCrossStrandReadGraphEdges1 and flagChimericReads (src/AssemblerReadGraph.cpp:355-583, 775-1041) ------------
+// Both take the read graph as shb_create_read_graph returns it (edges, ReadGraphConnectivity toc/data over 2*readCount
+// oriented reads) and work on any context (one that holds only a read range too). They are all-or-nothing: an error
+// leaves every in/out array unchanged. A connectivity entry that names an edge which does not exist or does not touch its
+// oriented read, or an edge whose oriented reads do not exist, returns SHB_ERR_INVALID (the reference's getOther asserts);
+// so does a readCount of 2^29 or more.
+// ballSizeHistogram[k] counts the reads whose search reached [2^k, 2^(k+1)) oriented reads (the work done); a read whose
+// search outgrows the shared-memory table is searched again with its table in device memory (overflowReadCount).
+typedef struct {
+    uint64_t nearStrandJumpReportedCount;   // the number the reference prints: isNearStrandJump[v] over v < readCount (:820-824)
+    uint64_t nearStrandJumpCount;           // oriented reads within maxDistance of their reverse complement
+    uint64_t regionCount;                   // strand jump regions (components of >= 2 vertices)
+    uint64_t crossStrandEdgeCount;          // edges flagged crossesStrands
+    uint64_t overflowReadCount;
+    double deviceMs;                        // wall time of the device part: the graph's checks and upload, the searches, the regions
+    double hostMs;                          // wall time of the per-region processing on the host
+    double totalMs;
+    uint64_t peakDeviceBytes;               // high-water mark of the device memory this call allocated
+    uint64_t ballSizeHistogram[32];
+} shb_cross_strand_result;
+/* Replaces Assembler::flagCrossStrandReadGraphEdges1(maxDistance) (ReadGraph.strandSeparationMethod 1): clears
+ * crossesStrands on every edge, then (maxDistance > 0) flags the edges that would join an oriented read to its reverse
+ * complement inside each strand jump region, processed by decreasing alignment markerCount, and clears
+ * AlignmentInfo::isInReadGraph of their alignments. Identical to the reference, including its order among pairs that tie
+ * on markerCount (std::sort of the same sequence).
+ *   readGraphEdges : IN/OUT, edgeCount 16-byte ReadGraphEdge records (crossesStrands is bit 62 of the second word).
+ *   alignmentData  : IN/OUT, alignmentCount 64-byte AlignmentData records (markerCount read, isInReadGraph cleared).
+ * A negative maxDistance returns SHB_ERR_INVALID, and so does a region that trips one of the reference's assertions (an odd
+ * number of vertices, vertices that are not the two strands of their reads, an odd number of edges, a pair of edges with
+ * different alignment ids, an oriented read already joined to its reverse complement) or names an alignment >= alignmentCount. */
+shb_status shb_flag_cross_strand_read_graph_edges1(shb_context* ctx, int64_t maxDistance, void* readGraphEdges, uint64_t edgeCount,
+                                                   const uint32_t* connectivityToc, const uint32_t* connectivityData, uint64_t readCount,
+                                                   void* alignmentData, uint64_t alignmentCount, shb_cross_strand_result* result);
+typedef struct {
+    uint64_t chimericReadCount;
+    uint64_t overflowReadCount;
+    double deviceMs;                        // wall time of the device part: the graph's checks and upload, the searches
+    double totalMs;
+    uint64_t peakDeviceBytes;
+    uint64_t ballSizeHistogram[32];
+} shb_chimeric_result;
+/* Replaces Assembler::flagChimericReads(maxDistance): read x is chimeric when the oriented reads at distance exactly
+ * maxDistance from x-0 (edges flagged crossesStrands skipped, x-1 left out) fall into two or more connected components once
+ * read x is removed. Rewrites the isChimeric bit (bit 1) of every readFlags byte and keeps the others; clears
+ * AlignmentInfo::isInReadGraph of every alignment of a chimeric read. maxDistance 0 clears every isChimeric bit; 255 or
+ * more returns SHB_ERR_INVALID (the reference asserts), and so does an alignment that names a read >= readCount. */
+shb_status shb_flag_chimeric_reads(shb_context* ctx, uint64_t maxDistance, const void* readGraphEdges, uint64_t edgeCount,
+                                   const uint32_t* connectivityToc, const uint32_t* connectivityData, uint64_t readCount,
+                                   uint8_t* readFlags, void* alignmentData, uint64_t alignmentCount, shb_chimeric_result* result);
+
 // ---- createMarkerGraphVertices (src/AssemblerMarkerGraph.cpp:38-770) ------------------------------------------------
 // The arguments of Assembler::createMarkerGraphVertices (defaults src/AssemblerOptions.cpp:577-685: 10, 100, 0, 0, 0.08,
 // 2). minCoverage 0 selects it from the disjoint-set size histogram with the reference's PeakFinder. threadCount is

@@ -343,6 +343,72 @@ class Assembler:
                                    toc_dtype=np.uint32, page_size=self.page_size)
         return int(keep.sum())
 
+    def _read_graph_for_flags(self):
+        """(edges, toc, data, alignment records) of this session's read graph, else of Data/ (writable copies)."""
+        if getattr(self, "_read_graph", None) is not None:
+            edges, toc, data = self._read_graph
+        else:
+            edges = mm_read_vector(self._name("ReadGraphEdges"), np.uint32, object_size=16)
+            toc = mm_read_vector(self._name("ReadGraphConnectivity.toc"), np.uint32)
+            data = mm_read_vector(self._name("ReadGraphConnectivity.data"), np.uint32, object_size=4)
+        if self._alignment_data is None:
+            raise RuntimeError("Alignment data are not accessible.")
+        rec = np.ascontiguousarray(np.array(self._alignment_data, np.uint32)).reshape(-1, 16)
+        return np.array(edges, np.uint32).reshape(-1, 4), np.asarray(toc, np.uint32), np.asarray(data, np.uint32), rec
+
+    def _store_read_graph_flags(self, edges, toc, data, rec):
+        self._alignment_data = rec
+        self._read_graph = (edges, toc, data)
+        self._read_graph_edges = edges
+        mm_write_vector(self._name("AlignmentData"), rec, object_size=64, page_size=self.page_size)
+        mm_write_vector(self._name("ReadGraphEdges"), edges, object_size=16, page_size=self.page_size)
+
+    def flagCrossStrandReadGraphEdges1(self, maxDistance, threadCount=0):
+        """Assembler::flagCrossStrandReadGraphEdges1 (src/AssemblerReadGraph.cpp:775-1041, binding src/PythonModule.cpp:388-393;
+        ReadGraph.strandSeparationMethod 1) on the device. Rewrites crossesStrands in Data/ReadGraphEdges and clears
+        AlignmentInfo::isInReadGraph in Data/AlignmentData for the edges it flags; the session's read graph is updated, so a
+        following createMarkerGraphVertices sees the flags. Prints the reference's lines. threadCount is ignored."""
+        from . import capi
+        edges, toc, data, rec = self._read_graph_for_flags()
+        try:
+            res = capi.flag_cross_strand_read_graph_edges1(self._context(), maxDistance, edges, toc, data, rec)
+        except capi.ShastaB200Error as e:
+            raise RuntimeError(str(e)) from None
+        self._store_read_graph_flags(edges, toc, data, rec)
+        self.crossStrandResult = res
+        if maxDistance == 0:
+            print("Skipped flagCrossStrandReadGraphEdges.")
+            return
+        print(f"Of {len(toc) - 1} vertices in the read graph, {res['nearStrandJumpReportedCount']} are within distance "
+              f"{maxDistance} of their reverse complement.")
+        print(f"Found {res['regionCount']} strand jump regions.")
+        print(f"Marked {res['crossStrandEdgeCount']} read graph edges out of {len(edges)} total as cross-strand.")
+
+    def flagChimericReads(self, maxChimericReadDistance, threadCount=0):
+        """Assembler::flagChimericReads (src/AssemblerReadGraph.cpp:355-583, binding src/PythonModule.cpp:394-397) on the
+        device. Rewrites the isChimeric bit of Data/ReadFlags and clears AlignmentInfo::isInReadGraph in Data/AlignmentData for
+        every alignment of a chimeric read. Prints the reference's lines. threadCount is ignored."""
+        from . import capi
+        edges, toc, data, rec = self._read_graph_for_flags()
+        if self._markers is not None:
+            flags = np.array(self._markers[2], np.uint8)
+        else:
+            flags = np.array(mm_read_vector(self._name("ReadFlags"), np.uint8, object_size=1), np.uint8)
+        try:
+            res = capi.flag_chimeric_reads(self._context(), maxChimericReadDistance, edges, toc, data, flags, rec)
+        except capi.ShastaB200Error as e:
+            raise RuntimeError(str(e)) from None
+        self._store_read_graph_flags(edges, toc, data, rec)
+        mm_write_vector(self._name("ReadFlags"), flags, object_size=1)
+        if self._markers is not None:
+            self._markers = (self._markers[0], self._markers[1], flags)
+        self.chimericResult = res
+        if maxChimericReadDistance == 0:
+            return
+        readCount = len(flags)
+        print(f"Flagged {res['chimericReadCount']} reads as chimeric out of {readCount} total.")
+        print(f"Chimera rate is {_ostream_double(res['chimericReadCount'] / readCount if readCount else float('nan'))}")
+
     # ------------------------------------------------------------------ the two hot-path entry points
     def findAlignmentCandidatesLowHash0(self, m, hashFraction, minHashIterationCount, alignmentCandidatesPerRead,
                                         minBucketSize, maxBucketSize, minFrequency, log2MinHashBucketCount=0, threadCount=0):

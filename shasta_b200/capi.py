@@ -487,6 +487,69 @@ def create_read_graph2(ctx: Context, records, read_count, max_alignment_count, m
     return crit.asdict(), keepn, edgesn, tocn, datan
 
 
+class CrossStrandResult(C.Structure):
+    _fields_ = [("nearStrandJumpReportedCount", C.c_uint64), ("nearStrandJumpCount", C.c_uint64), ("regionCount", C.c_uint64),
+                ("crossStrandEdgeCount", C.c_uint64), ("overflowReadCount", C.c_uint64), ("deviceMs", C.c_double),
+                ("hostMs", C.c_double), ("totalMs", C.c_double), ("peakDeviceBytes", C.c_uint64),
+                ("ballSizeHistogram", C.c_uint64 * 32)]
+
+    def asdict(self):
+        d = {k: getattr(self, k) for k, _ in self._fields_}
+        d["ballSizeHistogram"] = list(self.ballSizeHistogram)
+        return d
+
+
+class ChimericResult(C.Structure):
+    _fields_ = [("chimericReadCount", C.c_uint64), ("overflowReadCount", C.c_uint64), ("deviceMs", C.c_double), ("totalMs", C.c_double),
+                ("peakDeviceBytes", C.c_uint64), ("ballSizeHistogram", C.c_uint64 * 32)]
+
+    def asdict(self):
+        d = {k: getattr(self, k) for k, _ in self._fields_}
+        d["ballSizeHistogram"] = list(self.ballSizeHistogram)
+        return d
+
+
+def _writable(a, dtype):
+    assert a.dtype == dtype and a.flags["C_CONTIGUOUS"] and a.flags["WRITEABLE"]
+    return a
+
+
+def flag_cross_strand_read_graph_edges1(ctx: Context, max_distance, edges, connectivity_toc, connectivity_data, records):
+    """Assembler::flagCrossStrandReadGraphEdges1 (shb_flag_cross_strand_read_graph_edges1). edges uint32[E,4] and records
+    uint32[n,16] must be writable and C-contiguous: crossesStrands and AlignmentInfo::isInReadGraph are rewritten in place.
+    Returns the result dict. An error (negative max_distance, a reference assertion) raises ShastaB200Error and leaves both
+    arrays unchanged."""
+    _writable(edges, np.uint32)
+    _writable(records, np.uint32)
+    toc = np.ascontiguousarray(connectivity_toc, np.uint32)
+    data = np.ascontiguousarray(connectivity_data, np.uint32)
+    res = CrossStrandResult()
+    f = lib().shb_flag_cross_strand_read_graph_edges1
+    f.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
+                  C.POINTER(CrossStrandResult)]
+    _check(f(ctx._h, int(max_distance), _ptr(edges), edges.size // 4, _ptr(toc), _ptr(data), (len(toc) - 1) // 2, _ptr(records),
+             records.size // 16, C.byref(res)))
+    return res.asdict()
+
+
+def flag_chimeric_reads(ctx: Context, max_distance, edges, connectivity_toc, connectivity_data, read_flags, records):
+    """Assembler::flagChimericReads (shb_flag_chimeric_reads). read_flags uint8[R] and records uint32[n,16] must be writable
+    and C-contiguous: isChimeric (bit 1) and AlignmentInfo::isInReadGraph are rewritten in place. Returns the result dict.
+    max_distance >= 255 raises ShastaB200Error and leaves both arrays unchanged."""
+    _writable(read_flags, np.uint8)
+    _writable(records, np.uint32)
+    e = np.ascontiguousarray(edges, np.uint32)
+    toc = np.ascontiguousarray(connectivity_toc, np.uint32)
+    data = np.ascontiguousarray(connectivity_data, np.uint32)
+    res = ChimericResult()
+    f = lib().shb_flag_chimeric_reads
+    f.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                  C.c_uint64, C.POINTER(ChimericResult)]
+    _check(f(ctx._h, int(max_distance), _ptr(e), e.size // 4, _ptr(toc), _ptr(data), (len(toc) - 1) // 2, _ptr(read_flags),
+             _ptr(records), records.size // 16, C.byref(res)))
+    return res.asdict()
+
+
 def align_oriented_reads(ctx: Context, oriented_read_id0, oriented_read_id1, options: AlignOptions):
     """Single pair in the orientation given (shb_align_oriented_reads). Returns (ordinals uint32[n,2], info uint32[13])."""
     ords = C.c_void_p()

@@ -51,6 +51,12 @@ void createMarkerGraphVertices(shb_context* c, const shb_marker_graph_params& p,
                                shb_marker_graph_result* result);
 void findMarkerGraphReverseComplementVertices(shb_context* c, const uint8_t* table5, const uint8_t* toc5, const uint64_t* vdata,
                                               uint64_t V, uint64_t** rcOut);
+void flagCrossStrandReadGraphEdges1(shb_context* c, int64_t maxDistance, uint32_t* edges, uint64_t edgeCount, const uint32_t* connToc,
+                                    const uint32_t* connData, uint64_t readCount, uint32_t* rec, uint64_t alignmentCount,
+                                    shb_cross_strand_result* result);
+void flagChimericReads(shb_context* c, uint64_t maxDistance, const uint32_t* edges, uint64_t edgeCount, const uint32_t* connToc,
+                       const uint32_t* connData, uint64_t readCount, uint8_t* readFlags, uint32_t* rec, uint64_t alignmentCount,
+                       shb_chimeric_result* result);
 
 template<class F> shb_status guarded(F&& f)
 {
@@ -456,6 +462,30 @@ shb_status shb_palindromic_read_alignment(shb_context* c, uint64_t readId, const
     return guarded([&] {
         SHB_REQUIRE(c && params && ordinals && count, SHB_ERR_INVALID, "Null argument.");
         palindromicReadAlignment(c, readId, *params, ordinals, count);
+    });
+}
+
+shb_status shb_flag_cross_strand_read_graph_edges1(shb_context* c, int64_t maxDistance, void* readGraphEdges, uint64_t edgeCount,
+                                                   const uint32_t* connectivityToc, const uint32_t* connectivityData, uint64_t readCount,
+                                                   void* alignmentData, uint64_t alignmentCount, shb_cross_strand_result* result)
+{
+    return guarded([&] {
+        SHB_REQUIRE(c && (readGraphEdges || edgeCount == 0) && connectivityToc && (connectivityData || connectivityToc[2 * readCount] == 0) &&
+                    (alignmentData || alignmentCount == 0), SHB_ERR_INVALID, "Null argument.");
+        flagCrossStrandReadGraphEdges1(c, maxDistance, static_cast<uint32_t*>(readGraphEdges), edgeCount, connectivityToc, connectivityData,
+                                       readCount, static_cast<uint32_t*>(alignmentData), alignmentCount, result);
+    });
+}
+
+shb_status shb_flag_chimeric_reads(shb_context* c, uint64_t maxDistance, const void* readGraphEdges, uint64_t edgeCount,
+                                   const uint32_t* connectivityToc, const uint32_t* connectivityData, uint64_t readCount,
+                                   uint8_t* readFlags, void* alignmentData, uint64_t alignmentCount, shb_chimeric_result* result)
+{
+    return guarded([&] {
+        SHB_REQUIRE(c && (readGraphEdges || edgeCount == 0) && connectivityToc && (connectivityData || connectivityToc[2 * readCount] == 0) &&
+                    (readFlags || readCount == 0) && (alignmentData || alignmentCount == 0), SHB_ERR_INVALID, "Null argument.");
+        flagChimericReads(c, maxDistance, static_cast<const uint32_t*>(readGraphEdges), edgeCount, connectivityToc, connectivityData,
+                          readCount, readFlags, static_cast<uint32_t*>(alignmentData), alignmentCount, result);
     });
 }
 
