@@ -22,24 +22,29 @@ class ShastaB200Error(RuntimeError):
         self.status = status
 
 
-class LowHashParams(C.Structure):
+class _Struct(C.Structure):
+    """Base of the ctypes mirrors of the structs of include/shasta_b200.h."""
+
+    def asdict(self):
+        """Field name -> value; array fields become lists."""
+        return {k: list(v) if isinstance(v, C.Array) else v for k, v in ((k, getattr(self, k)) for k, _ in self._fields_)}
+
+
+class LowHashParams(_Struct):
     _fields_ = [("m", C.c_uint64), ("hashFraction", C.c_double), ("minHashIterationCount", C.c_uint64),
                 ("alignmentCandidatesPerRead", C.c_double), ("log2MinHashBucketCount", C.c_uint64),
                 ("minBucketSize", C.c_uint64), ("maxBucketSize", C.c_uint64), ("minFrequency", C.c_uint64),
                 ("threadCount", C.c_uint64), ("perIterationMerge", C.c_uint32), ("reserved", C.c_uint32)]
 
 
-class LowHashResult(C.Structure):
+class LowHashResult(_Struct):
     _fields_ = [("iterations", C.c_uint64), ("log2BucketCount", C.c_uint64), ("lowHashCount", C.c_uint64),
                 ("pairCount", C.c_uint64), ("candidateCount", C.c_uint64), ("sweepMs", C.c_double),
                 ("totalMs", C.c_double), ("sweepLaunches", C.c_uint64), ("kernelLaunches", C.c_uint64),
                 ("candidateDigest", C.c_uint64)]
 
-    def asdict(self):
-        return {k: getattr(self, k) for k, _ in self._fields_}
 
-
-class AlignOptions(C.Structure):
+class AlignOptions(_Struct):
     """shb_align_options: AlignOptions of src/AssemblerOptions.hpp:177-199 + k."""
     _fields_ = [("alignMethod", C.c_int32), ("maxSkip", C.c_int32), ("maxDrift", C.c_int32), ("maxTrim", C.c_int32),
                 ("maxMarkerFrequency", C.c_int32), ("minAlignedMarkerCount", C.c_int32), ("minAlignedFraction", C.c_double),
@@ -50,7 +55,7 @@ class AlignOptions(C.Structure):
                 ("align4MaxDistanceFromBoundary", C.c_uint64), ("k", C.c_uint32), ("reserved", C.c_uint32)]
 
 
-class AlignResult(C.Structure):
+class AlignResult(_Struct):
     _fields_ = [("candidateCount", C.c_uint64), ("alignmentCount", C.c_uint64), ("skippedCount", C.c_uint64),
                 ("dpCells", C.c_uint64), ("dpMs", C.c_double), ("totalMs", C.c_double), ("kernelLaunches", C.c_uint64),
                 ("outputCopyMs", C.c_double), ("hostWallMs", C.c_double), ("dpUsefulCells", C.c_uint64),
@@ -58,18 +63,15 @@ class AlignResult(C.Structure):
                 ("compressedDigest", C.c_uint64)]
 
 
-class MarkerResult(C.Structure):
+class MarkerResult(_Struct):
     _fields_ = [("readCount", C.c_uint64), ("baseCount", C.c_uint64), ("markerCount", C.c_uint64), ("totalMs", C.c_double),
                 ("kernelLaunches", C.c_uint64), ("h2dBytes", C.c_uint64)]
 
 
-class DistTiming(C.Structure):
+class DistTiming(_Struct):
     _fields_ = [("sweepSeconds", C.c_double), ("partitionSeconds", C.c_double), ("exchangeSeconds", C.c_double),
                 ("processSeconds", C.c_double), ("finalSeconds", C.c_double), ("gatherSeconds", C.c_double),
                 ("totalSeconds", C.c_double), ("entriesReceived", C.c_uint64), ("pairsReceived", C.c_uint64)]
-
-    def asdict(self):
-        return {k: getattr(self, k) for k, _ in self._fields_}
 
 
 # Defaults of src/AssemblerOptions.cpp:380-489
@@ -152,6 +154,25 @@ def lib():
         L.shb_lowhash_stats_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
         L.shb_lowhash_counters.argtypes = [C.c_void_p, C.POINTER(LowHashResult)]
         L.shb_copy_device_to_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
+        L.shb_test_radix_sort.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_int]
+        L.shb_create_read_graph2.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_double, C.c_double,
+                                             C.c_double, C.c_double, C.c_double, C.POINTER(ReadGraph2Criteria), C.POINTER(C.c_void_p),
+                                             C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
+        L.shb_flag_cross_strand_read_graph_edges1.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                                                              C.c_uint64, C.c_void_p, C.c_uint64, C.POINTER(CrossStrandResult)]
+        L.shb_flag_chimeric_reads.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64,
+                                              C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(ChimericResult)]
+        L.shb_flag_palindromic_reads.argtypes = [C.c_void_p, C.POINTER(PalindromicParams), C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.POINTER(PalindromicResult)]
+        L.shb_palindromic_read_alignment.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(PalindromicParams), C.POINTER(C.c_void_p),
+                                                     C.POINTER(C.c_uint64)]
+        L.shb_create_marker_graph_vertices.argtypes = [C.c_void_p, C.POINTER(MarkerGraphParams), C.c_void_p, C.c_uint64, C.c_void_p,
+                                                       C.c_void_p, C.c_uint64, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                                       C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(MarkerGraphResult)]
+        L.shb_find_marker_graph_reverse_complement_vertices.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
+                                                                        C.POINTER(C.c_void_p)]
+        L.shb_peak_finder_cutoff.restype = C.c_int
+        L.shb_peak_finder_cutoff.argtypes = [C.c_void_p, C.c_uint64, C.c_double, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_double)]
         _lib = L
     return _lib
 
@@ -203,12 +224,8 @@ class Context:
         self.read_count = R
         if not want_host:
             return None, None, res
-        tocn = np.ctypeslib.as_array(C.cast(toc, C.POINTER(C.c_uint64)), (2 * R + 1,)).copy()
-        M = int(tocn[-1])
-        datan = np.ctypeslib.as_array(C.cast(data, C.POINTER(C.c_uint8)), (7 * M,)).copy() if M else np.zeros(0, np.uint8)
-        lib().shb_free(toc)
-        lib().shb_free(data)
-        return tocn, datan, res
+        tocn = _owned_array(toc, 2 * R + 1, np.uint64)
+        return tocn, _owned_array(data, 7 * int(tocn[-1]), np.uint8), res
 
     # ---- multi-GPU (one process per GPU; NCCL inside the library) -------------------------------------------------
     def dist_init(self, world, rank, unique_id: bytes):
@@ -240,35 +257,29 @@ class Context:
         except Exception:
             pass
 
+    @staticmethod
+    def _marker_range(toc, read_begin, read_end, read_count_total, total_marker_count):
+        """(readCountTotal, readBegin, readEnd, totalMarkerCount) of shb_set_markers*: by default toc holds every read."""
+        n_local = (len(toc) - 1) // 2
+        return (n_local if read_count_total is None else read_count_total, read_begin,
+                read_begin + n_local if read_end is None else read_end, int(toc[-1]) if total_marker_count is None else total_marker_count)
+
     def set_markers(self, toc, data7, flags, read_begin=0, read_end=None, read_count_total=None, total_marker_count=None):
         toc = np.ascontiguousarray(toc, dtype=np.uint64)
         data7 = np.ascontiguousarray(data7, dtype=np.uint8)
         flags = np.ascontiguousarray(flags, dtype=np.uint8)
-        n_local = (len(toc) - 1) // 2
-        if read_count_total is None:
-            read_count_total = n_local
-        if read_end is None:
-            read_end = read_begin + n_local
-        if total_marker_count is None:
-            total_marker_count = int(toc[-1])
-        _check(lib().shb_set_markers(self._h, read_count_total, read_begin, read_end, _ptr(toc), _ptr(data7), _ptr(flags), total_marker_count))
-        self.read_count = read_count_total
+        total, begin, end, markers = self._marker_range(toc, read_begin, read_end, read_count_total, total_marker_count)
+        _check(lib().shb_set_markers(self._h, total, begin, end, _ptr(toc), _ptr(data7), _ptr(flags), markers))
+        self.read_count = total
 
     def set_markers_device(self, toc, kmer_ids_device_ptr, flags, keepalive=None, read_begin=0, read_end=None,
                            read_count_total=None, total_marker_count=None):
         toc = np.ascontiguousarray(toc, dtype=np.uint64)
         flags = np.ascontiguousarray(flags, dtype=np.uint8)
-        n_local = (len(toc) - 1) // 2
-        if read_count_total is None:
-            read_count_total = n_local
-        if read_end is None:
-            read_end = read_begin + n_local
-        if total_marker_count is None:
-            total_marker_count = int(toc[-1])
-        _check(lib().shb_set_markers_device(self._h, read_count_total, read_begin, read_end, _ptr(toc),
-                                            C.c_void_p(kmer_ids_device_ptr), _ptr(flags), total_marker_count))
+        total, begin, end, markers = self._marker_range(toc, read_begin, read_end, read_count_total, total_marker_count)
+        _check(lib().shb_set_markers_device(self._h, total, begin, end, _ptr(toc), C.c_void_p(kmer_ids_device_ptr), _ptr(flags), markers))
         self._keep = keepalive
-        self.read_count = read_count_total
+        self.read_count = total
 
     def lowhash0(self, params: LowHashParams, want_stats=True, max_iter_summary=0):
         """Returns (candidates uint32[n,3] = (readId0, readId1, isSameStrand), stats uint64[R,3] | None,
@@ -379,23 +390,26 @@ def candidates_to_records(cand):
     return np.ascontiguousarray(cand, dtype=np.uint32).reshape(-1, 3)
 
 
-def compute_alignments(ctx: Context, candidates, options: AlignOptions):
-    """Assembler::computeAlignments on the markers held by ctx.
-    Returns (records uint32[count,16], compressedToc uint64[count+1], compressedData uint8[], AlignResult)."""
+def _compute_alignments(f, ctx: Context, candidates, options: AlignOptions):
     cand = candidates_to_records(candidates)
     rec = C.c_void_p()
     cnt = C.c_uint64()
     toc = C.c_void_p()
     data = C.c_void_p()
     res = AlignResult()
-    _check(lib().shb_compute_alignments(ctx._h, _ptr(cand), len(cand), C.byref(options), C.byref(rec), C.byref(cnt),
-                                        C.byref(toc), C.byref(data), C.byref(res)))
+    _check(f(ctx._h, _ptr(cand), len(cand), C.byref(options), C.byref(rec), C.byref(cnt), C.byref(toc), C.byref(data), C.byref(res)))
     n = cnt.value
     tocn = _owned_array(toc, n + 1, np.uint64)
     nb = int(tocn[-1])
     records = _owned_array(rec, 16 * n, np.uint32).reshape(n, 16)
     datan = _owned_array(data, nb, np.uint8)
     return records, tocn, datan, res
+
+
+def compute_alignments(ctx: Context, candidates, options: AlignOptions):
+    """Assembler::computeAlignments on the markers held by ctx.
+    Returns (records uint32[count,16], compressedToc uint64[count+1], compressedData uint8[], AlignResult)."""
+    return _compute_alignments(lib().shb_compute_alignments, ctx, candidates, options)
 
 
 def dist_unique_id() -> bytes:
@@ -408,20 +422,7 @@ def dist_unique_id() -> bytes:
 def compute_alignments_sharded(ctx: Context, candidates, options: AlignOptions):
     """Assembler::computeAlignments on this rank's block of candidates; the k-mer ids of all ranks are gathered into this
     GPU on the first call after the markers changed (collective then). Same returns as compute_alignments."""
-    cand = candidates_to_records(candidates)
-    rec = C.c_void_p()
-    cnt = C.c_uint64()
-    toc = C.c_void_p()
-    data = C.c_void_p()
-    res = AlignResult()
-    _check(lib().shb_compute_alignments_sharded(ctx._h, _ptr(cand), len(cand), C.byref(options), C.byref(rec), C.byref(cnt),
-                                                C.byref(toc), C.byref(data), C.byref(res)))
-    n = cnt.value
-    tocn = _owned_array(toc, n + 1, np.uint64)
-    nb = int(tocn[-1])
-    records = _owned_array(rec, 16 * n, np.uint32).reshape(n, 16)
-    datan = _owned_array(data, nb, np.uint8)
-    return records, tocn, datan, res
+    return _compute_alignments(lib().shb_compute_alignments_sharded, ctx, candidates, options)
 
 
 def compute_alignment_table(ctx: Context, records, read_count):
@@ -430,11 +431,7 @@ def compute_alignment_table(ctx: Context, records, read_count):
     toc = C.c_void_p()
     data = C.c_void_p()
     _check(lib().shb_compute_alignment_table(ctx._h, _ptr(rec), len(rec), read_count, C.byref(toc), C.byref(data)))
-    tocn = np.ctypeslib.as_array(C.cast(toc, C.POINTER(C.c_uint32)), (2 * read_count + 1,)).copy()
-    datan = np.ctypeslib.as_array(C.cast(data, C.POINTER(C.c_uint32)), (4 * len(rec),)).copy() if len(rec) else np.zeros(0, np.uint32)
-    lib().shb_free(toc)
-    lib().shb_free(data)
-    return tocn, datan
+    return _owned_array(toc, 2 * read_count + 1, np.uint32), _owned_array(data, 4 * len(rec), np.uint32)
 
 
 def create_read_graph(ctx: Context, records, read_count, max_alignment_count):
@@ -443,70 +440,48 @@ def create_read_graph(ctx: Context, records, read_count, max_alignment_count):
     Returns (keep uint8[n], edges uint32[E,4] = 16-byte ReadGraphEdge records, connectivityToc uint32[2R+1], connectivityData uint32[2E]);
     each connectivity row lists its edges in decreasing edge index, the reference's order. A kept alignment whose edge is not
     ordered (readIds[0] > readIds[1], or a read aligned to itself) raises ShastaB200Error (SHB_ERR_INVALID), records untouched."""
+    return _read_graph(records, read_count, lambda rec, *out: lib().shb_create_read_graph(
+        ctx._h, _ptr(rec), len(rec), int(read_count), int(max_alignment_count), *out))
+
+
+def _read_graph(records, read_count, call):
+    """call(rec, keep, edges, edgeCount, connectivityToc, connectivityData) with the outputs by reference; returns the four arrays."""
     assert records.dtype == np.uint32 and records.flags["C_CONTIGUOUS"] and records.flags["WRITEABLE"]
     rec = records.reshape(-1, 16)
     keep, edges, toc, data = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
     e = C.c_uint64()
-    _check(lib().shb_create_read_graph(ctx._h, _ptr(rec), len(rec), int(read_count), int(max_alignment_count), C.byref(keep), C.byref(edges),
-                                       C.byref(e), C.byref(toc), C.byref(data)))
-    keepn = _owned_array(keep, len(rec), np.uint8)
-    edgesn = _owned_array(edges, 4 * e.value, np.uint32).reshape(-1, 4)
-    tocn = _owned_array(toc, 2 * int(read_count) + 1, np.uint32)
-    datan = _owned_array(data, 2 * e.value, np.uint32)
-    return keepn, edgesn, tocn, datan
+    _check(call(rec, C.byref(keep), C.byref(edges), C.byref(e), C.byref(toc), C.byref(data)))
+    return (_owned_array(keep, len(rec), np.uint8), _owned_array(edges, 4 * e.value, np.uint32).reshape(-1, 4),
+            _owned_array(toc, 2 * int(read_count) + 1, np.uint32), _owned_array(data, 2 * e.value, np.uint32))
 
 
-class ReadGraph2Criteria(C.Structure):
+class ReadGraph2Criteria(_Struct):
     _fields_ = [("minAlignedFraction", C.c_double), ("minAlignedMarkerCount", C.c_uint64), ("maxDrift", C.c_uint64),
                 ("maxSkip", C.c_uint64), ("maxTrim", C.c_uint64)]
-
-    def asdict(self):
-        return {k: getattr(self, k) for k, _ in self._fields_}
 
 
 def create_read_graph2(ctx: Context, records, read_count, max_alignment_count, marker_count_percentile, aligned_fraction_percentile,
                        max_skip_percentile, max_drift_percentile, max_trim_percentile):
     """Assembler::createReadGraph2, ReadGraph.creationMethod 2 (shb_create_read_graph2). records as in create_read_graph.
     Returns (criteria dict, keep, edges, connectivityToc, connectivityData), and refuses what create_read_graph refuses."""
-    assert records.dtype == np.uint32 and records.flags["C_CONTIGUOUS"] and records.flags["WRITEABLE"]
-    rec = records.reshape(-1, 16)
-    keep, edges, toc, data = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
-    e = C.c_uint64()
     crit = ReadGraph2Criteria()
-    f = lib().shb_create_read_graph2
-    f.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double,
-                  C.POINTER(ReadGraph2Criteria), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64),
-                  C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-    _check(f(ctx._h, _ptr(rec), len(rec), int(read_count), int(max_alignment_count), float(marker_count_percentile),
-             float(aligned_fraction_percentile), float(max_skip_percentile), float(max_drift_percentile), float(max_trim_percentile),
-             C.byref(crit), C.byref(keep), C.byref(edges), C.byref(e), C.byref(toc), C.byref(data)))
-    keepn = _owned_array(keep, len(rec), np.uint8)
-    edgesn = _owned_array(edges, 4 * e.value, np.uint32).reshape(-1, 4)
-    tocn = _owned_array(toc, 2 * int(read_count) + 1, np.uint32)
-    datan = _owned_array(data, 2 * e.value, np.uint32)
-    return crit.asdict(), keepn, edgesn, tocn, datan
+    graph = _read_graph(records, read_count, lambda rec, *out: lib().shb_create_read_graph2(
+        ctx._h, _ptr(rec), len(rec), int(read_count), int(max_alignment_count), float(marker_count_percentile),
+        float(aligned_fraction_percentile), float(max_skip_percentile), float(max_drift_percentile), float(max_trim_percentile),
+        C.byref(crit), *out))
+    return (crit.asdict(),) + graph
 
 
-class CrossStrandResult(C.Structure):
+class CrossStrandResult(_Struct):
     _fields_ = [("nearStrandJumpReportedCount", C.c_uint64), ("nearStrandJumpCount", C.c_uint64), ("regionCount", C.c_uint64),
                 ("crossStrandEdgeCount", C.c_uint64), ("overflowReadCount", C.c_uint64), ("deviceMs", C.c_double),
                 ("hostMs", C.c_double), ("totalMs", C.c_double), ("peakDeviceBytes", C.c_uint64),
                 ("ballSizeHistogram", C.c_uint64 * 32)]
 
-    def asdict(self):
-        d = {k: getattr(self, k) for k, _ in self._fields_}
-        d["ballSizeHistogram"] = list(self.ballSizeHistogram)
-        return d
 
-
-class ChimericResult(C.Structure):
+class ChimericResult(_Struct):
     _fields_ = [("chimericReadCount", C.c_uint64), ("overflowReadCount", C.c_uint64), ("deviceMs", C.c_double), ("totalMs", C.c_double),
                 ("peakDeviceBytes", C.c_uint64), ("ballSizeHistogram", C.c_uint64 * 32)]
-
-    def asdict(self):
-        d = {k: getattr(self, k) for k, _ in self._fields_}
-        d["ballSizeHistogram"] = list(self.ballSizeHistogram)
-        return d
 
 
 def _writable(a, dtype):
@@ -524,11 +499,8 @@ def flag_cross_strand_read_graph_edges1(ctx: Context, max_distance, edges, conne
     toc = np.ascontiguousarray(connectivity_toc, np.uint32)
     data = np.ascontiguousarray(connectivity_data, np.uint32)
     res = CrossStrandResult()
-    f = lib().shb_flag_cross_strand_read_graph_edges1
-    f.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
-                  C.POINTER(CrossStrandResult)]
-    _check(f(ctx._h, int(max_distance), _ptr(edges), edges.size // 4, _ptr(toc), _ptr(data), (len(toc) - 1) // 2, _ptr(records),
-             records.size // 16, C.byref(res)))
+    _check(lib().shb_flag_cross_strand_read_graph_edges1(ctx._h, int(max_distance), _ptr(edges), edges.size // 4, _ptr(toc), _ptr(data),
+                                                         (len(toc) - 1) // 2, _ptr(records), records.size // 16, C.byref(res)))
     return res.asdict()
 
 
@@ -542,11 +514,8 @@ def flag_chimeric_reads(ctx: Context, max_distance, edges, connectivity_toc, con
     toc = np.ascontiguousarray(connectivity_toc, np.uint32)
     data = np.ascontiguousarray(connectivity_data, np.uint32)
     res = ChimericResult()
-    f = lib().shb_flag_chimeric_reads
-    f.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
-                  C.c_uint64, C.POINTER(ChimericResult)]
-    _check(f(ctx._h, int(max_distance), _ptr(e), e.size // 4, _ptr(toc), _ptr(data), (len(toc) - 1) // 2, _ptr(read_flags),
-             _ptr(records), records.size // 16, C.byref(res)))
+    _check(lib().shb_flag_chimeric_reads(ctx._h, int(max_distance), _ptr(e), e.size // 4, _ptr(toc), _ptr(data), (len(toc) - 1) // 2,
+                                         _ptr(read_flags), _ptr(records), records.size // 16, C.byref(res)))
     return res.asdict()
 
 
@@ -557,13 +526,7 @@ def align_oriented_reads(ctx: Context, oriented_read_id0, oriented_read_id1, opt
     info = np.zeros(13, np.uint32)
     _check(lib().shb_align_oriented_reads(ctx._h, int(oriented_read_id0), int(oriented_read_id1), C.byref(options), C.byref(ords),
                                           C.byref(n), _ptr(info)))
-    if not ords or n.value == 0:
-        if ords:
-            lib().shb_free(ords)
-        return np.zeros((0, 2), np.uint32), info
-    out = np.ctypeslib.as_array(C.cast(ords, C.POINTER(C.c_uint32)), (n.value, 2)).copy()
-    lib().shb_free(ords)
-    return out, info
+    return _owned_array(ords, 2 * n.value, np.uint32).reshape(-1, 2), info
 
 
 def compute_candidate_table(ctx: Context, candidates, read_count):
@@ -572,11 +535,7 @@ def compute_candidate_table(ctx: Context, candidates, read_count):
     toc = C.c_void_p()
     data = C.c_void_p()
     _check(lib().shb_compute_candidate_table(ctx._h, _ptr(cand), len(cand), read_count, C.byref(toc), C.byref(data)))
-    tocn = np.ctypeslib.as_array(C.cast(toc, C.POINTER(C.c_uint64)), (2 * read_count + 1,)).copy()
-    datan = np.ctypeslib.as_array(C.cast(data, C.POINTER(C.c_uint64)), (4 * len(cand),)).copy() if len(cand) else np.zeros(0, np.uint64)
-    lib().shb_free(toc)
-    lib().shb_free(data)
-    return tocn, datan
+    return _owned_array(toc, 2 * read_count + 1, np.uint64), _owned_array(data, 4 * len(cand), np.uint64)
 
 
 def digest_records(records, words):
@@ -608,20 +567,17 @@ def _records_to_array(ptr, n):
 
 
 # ---- flagPalindromicReads (shb_flag_palindromic_reads) ---------------------------------------------------------------
-class PalindromicParams(C.Structure):
+class PalindromicParams(_Struct):
     """shb_palindromic_params: the arguments of Assembler::flagPalindromicReads (threadCount is ignored)."""
     _fields_ = [("maxSkip", C.c_uint32), ("maxDrift", C.c_uint32), ("maxMarkerFrequency", C.c_uint32), ("deltaThreshold", C.c_uint32),
                 ("alignedFractionThreshold", C.c_double), ("nearDiagonalFractionThreshold", C.c_double), ("threadCount", C.c_uint64)]
 
 
-class PalindromicResult(C.Structure):
+class PalindromicResult(_Struct):
     _fields_ = [("readCount", C.c_uint64), ("palindromicReadCount", C.c_uint64), ("exactReadCount", C.c_uint64),
                 ("vertexCount", C.c_uint64), ("edgeCount", C.c_uint64), ("heapPushCount", C.c_uint64),
                 ("heapsortFallbackCount", C.c_uint64), ("totalMs", C.c_double), ("exactMs", C.c_double),
                 ("kernelLaunches", C.c_uint64)]
-
-    def asdict(self):
-        return {k: getattr(self, k) for k, _ in self._fields_}
 
 
 def make_palindromic_params(maxSkip=100, maxDrift=100, maxMarkerFrequency=10, alignedFractionThreshold=0.1,
@@ -635,51 +591,38 @@ def flag_palindromic_reads(ctx: Context, params: PalindromicParams, read_flags=N
     """Flags palindromic reads on the markers ctx holds. read_flags (uint8[R], optional) is updated in place (bit 0 only).
     Returns (aligned uint32[R] or None, nearDiagonal uint32[R] or None, PalindromicResult). For reads decided without an
     alignment the counts are the prefilter's bounds (see include/shasta_b200.h)."""
-    L = lib()
-    f = L.shb_flag_palindromic_reads
-    f.argtypes = [C.c_void_p, C.POINTER(PalindromicParams), C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(PalindromicResult)]
     R = ctx.read_count
     aligned = np.zeros(R, np.uint32) if want_counts else None
     near = np.zeros(R, np.uint32) if want_counts else None
     if read_flags is not None:
         assert read_flags.dtype == np.uint8 and read_flags.flags["C_CONTIGUOUS"] and len(read_flags) == R
     res = PalindromicResult()
-    _check(f(ctx._h, C.byref(params), None if read_flags is None else read_flags.ctypes.data,
-             None if aligned is None else aligned.ctypes.data, None if near is None else near.ctypes.data, C.byref(res)))
+    _check(lib().shb_flag_palindromic_reads(ctx._h, C.byref(params), _ptr(read_flags), _ptr(aligned), _ptr(near), C.byref(res)))
     return aligned, near, res
 
 
 def palindromic_read_alignment(ctx: Context, read_id, params: PalindromicParams):
     """The alignment of read_id against its reverse complement (method 0). Returns ordinals uint32[n,2]."""
-    L = lib()
-    f = L.shb_palindromic_read_alignment
-    f.argtypes = [C.c_void_p, C.c_uint64, C.POINTER(PalindromicParams), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
     ords = C.c_void_p()
     n = C.c_uint64()
-    _check(f(ctx._h, int(read_id), C.byref(params), C.byref(ords), C.byref(n)))
-    out = np.ctypeslib.as_array(C.cast(ords, C.POINTER(C.c_uint32)), (n.value, 2)).copy() if n.value else np.zeros((0, 2), np.uint32)
-    if ords:
-        L.shb_free(ords)
-    return out
+    _check(lib().shb_palindromic_read_alignment(ctx._h, int(read_id), C.byref(params), C.byref(ords), C.byref(n)))
+    return _owned_array(ords, 2 * n.value, np.uint32).reshape(-1, 2)
 
 
 # ---- createMarkerGraphVertices (shb_create_marker_graph_vertices) ----------------------------------------------------
-class MarkerGraphParams(C.Structure):
+class MarkerGraphParams(_Struct):
     """shb_marker_graph_params: the arguments of Assembler::createMarkerGraphVertices (threadCount is ignored)."""
     _fields_ = [("minCoverage", C.c_uint64), ("maxCoverage", C.c_uint64), ("minCoveragePerStrand", C.c_uint64),
                 ("allowDuplicateMarkers", C.c_uint64), ("peakFinderMinAreaFraction", C.c_double),
                 ("peakFinderAreaStartIndex", C.c_uint64), ("threadCount", C.c_uint64)]
 
 
-class MarkerGraphResult(C.Structure):
+class MarkerGraphResult(_Struct):
     _fields_ = [("markerCount", C.c_uint64), ("minCoverageUsed", C.c_uint64), ("peakFinderFailed", C.c_uint64),
                 ("peakFinderObservedAreaFraction", C.c_double), ("edgePairsUsed", C.c_uint64), ("edgePairsSkipped", C.c_uint64),
                 ("alignedMarkerPairs", C.c_uint64), ("disjointSetCount", C.c_uint64), ("keptDisjointSetCount", C.c_uint64),
                 ("badDisjointSetCount", C.c_uint64), ("vertexCount", C.c_uint64), ("histogramSize", C.c_uint64),
                 ("peakDeviceBytes", C.c_uint64), ("deviceMs", C.c_double), ("totalMs", C.c_double), ("kernelLaunches", C.c_uint64)]
-
-    def asdict(self):
-        return {k: getattr(self, k) for k, _ in self._fields_}
 
 
 def make_marker_graph_params(minCoverage=10, maxCoverage=100, minCoveragePerStrand=0, allowDuplicateMarkers=False,
@@ -705,19 +648,14 @@ def create_marker_graph_vertices(ctx: Context, params: MarkerGraphParams, edges,
     """Assembler::createMarkerGraphVertices on the markers ctx holds. edges: uint32[E,4] ReadGraphEdge records.
     Returns (vertexTable uint8[5M] (Uint40), verticesToc uint8[5(V+1)] (Uint40), verticesData uint64[], histogram uint64[],
     MarkerGraphResult)."""
-    L = lib()
-    f = L.shb_create_marker_graph_vertices
-    f.argtypes = [C.c_void_p, C.POINTER(MarkerGraphParams), C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
-                  C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
-                  C.POINTER(MarkerGraphResult)]
     e = np.ascontiguousarray(edges, np.uint32).reshape(-1, 4)
     t = np.ascontiguousarray(compressed_toc, np.uint64)
     d = np.ascontiguousarray(compressed_data, np.uint8)
     fl = np.ascontiguousarray(read_flags, np.uint8)
     table, vtoc, vdata, hist = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
     res = MarkerGraphResult()
-    _check(f(ctx._h, C.byref(params), _ptr(e), len(e), _ptr(t), _ptr(d), len(t) - 1, _ptr(fl), C.byref(table), C.byref(vtoc),
-             C.byref(vdata), C.byref(hist), C.byref(res)))
+    _check(lib().shb_create_marker_graph_vertices(ctx._h, C.byref(params), _ptr(e), len(e), _ptr(t), _ptr(d), len(t) - 1, _ptr(fl),
+                                                  C.byref(table), C.byref(vtoc), C.byref(vdata), C.byref(hist), C.byref(res)))
     V = res.vertexCount
     tocn = _owned_array(vtoc, 5 * (V + 1), np.uint8)
     n = int(uint40_to_uint64(tocn)[-1]) if V else 0
@@ -729,25 +667,18 @@ def create_marker_graph_vertices(ctx: Context, params: MarkerGraphParams, edges,
 
 def find_marker_graph_reverse_complement_vertices(ctx: Context, vertex_table, vertices_toc, vertices_data):
     """Assembler::findMarkerGraphReverseComplementVertices. vertex_table / vertices_toc: Uint40 bytes. Returns uint64[V]."""
-    L = lib()
-    f = L.shb_find_marker_graph_reverse_complement_vertices
-    f.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_void_p)]
     t = np.ascontiguousarray(vertex_table, np.uint8)
     vt = np.ascontiguousarray(vertices_toc, np.uint8)
     vd = np.ascontiguousarray(vertices_data, np.uint64)
     V = len(vt) // 5 - 1
     rc = C.c_void_p()
-    _check(f(ctx._h, _ptr(t), _ptr(vt), _ptr(vd), V, C.byref(rc)))
+    _check(lib().shb_find_marker_graph_reverse_complement_vertices(ctx._h, _ptr(t), _ptr(vt), _ptr(vd), V, C.byref(rc)))
     return _owned_array(rc, V, np.uint64)
 
 
 def peak_finder_cutoff(histogram, min_area_fraction=0.08, start_index=2):
     """The library's PeakFinder restatement (host only). Returns (threw, cutoff, observedPercentArea)."""
-    L = lib()
-    f = L.shb_peak_finder_cutoff
-    f.restype = C.c_int
-    f.argtypes = [C.c_void_p, C.c_uint64, C.c_double, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_double)]
     y = np.ascontiguousarray(histogram, np.uint64)
     cutoff, observed = C.c_uint64(0), C.c_double(0)
-    threw = f(_ptr(y) if len(y) else None, len(y), float(min_area_fraction), int(start_index), C.byref(cutoff), C.byref(observed))
+    threw = lib().shb_peak_finder_cutoff(_ptr(y) if len(y) else None, len(y), float(min_area_fraction), int(start_index), C.byref(cutoff), C.byref(observed))
     return int(threw), int(cutoff.value), float(observed.value)

@@ -25,20 +25,6 @@ extern thread_local uint64_t g_launchCount;
 
 namespace {
 
-template<class T> T readBack(const T* dev, cudaStream_t st)
-{
-    T v;
-    SHB_CUDA(cudaMemcpyAsync(&v, dev, sizeof(T), cudaMemcpyDeviceToHost, st));
-    SHB_CUDA(cudaStreamSynchronize(st));
-    return v;
-}
-
-struct Events {
-    cudaEvent_t a = nullptr, b = nullptr;
-    Events() { cudaEventCreate(&a); cudaEventCreate(&b); }
-    ~Events() { cudaEventDestroy(a); cudaEventDestroy(b); }
-};
-
 // One launch per band class (dpClassAt). Wavefront classes run on groups of lanes in blocks of kDpMaxWarpsPerBlock
 // warps, with no shared memory; the scan kernel (c = 0) takes as many warps as fit its shared memory.
 uint32_t warpsForClass(const DpClass& k)
@@ -255,7 +241,7 @@ void buildDownsampled(shb_context* c, uint32_t k, double factor)
     c->indexBuf.reserve(std::min<uint64_t>(chunk, M) + 1);
     c->scanWs.reserve(scanWorkspaceElements(chunk));
     // scalars: 512 entries, allocated once at context creation
-    uint32_t* totalDev = reinterpret_cast<uint32_t*>(c->scalars.get() + 32);
+    uint32_t* totalDev = reinterpret_cast<uint32_t*>(c->scalar(kSlotDownsampleTotal));
     // Pass 0 sizes the output exactly; pass 1 compacts.
     uint64_t total = 0;
     for(int pass = 0; pass < 2; pass++) {
@@ -313,8 +299,7 @@ void buildSortedMarkers(shb_context* c, uint32_t k)
             keysA.reserve(n); keysB.reserve(n); valsA.reserve(n); valsB.reserve(n);
             SHB_LAUNCH(sortedMarkerKeysKernel, ceilDiv(n, 256), 256, 0, st, c->kmerIds, (const uint64_t*)c->toc.get(),
                        rowBegin, rowEnd, markerBegin, n, keysA.get(), valsA.get());
-            uint32_t rowBits = 1;
-            while((1ull << rowBits) < uint64_t(rowEnd - rowBegin)) rowBits++;
+            const uint32_t rowBits = bitsFor(rowEnd - rowBegin - 1);
             const int ranges[2][2] = {{0, int(2 * k)}, {32, 32 + int(rowBits)}};
             const bool inB = radixSort<true>(keysA.get(), keysB.get(), valsA.get(), valsB.get(), n, ranges, 2, c->sortWs, st);
             SHB_LAUNCH(sortedMarkerUnpackKernel, ceilDiv(n, 256), 256, 0, st, (const uint64_t*)(inB ? keysB.get() : keysA.get()), n,
@@ -694,7 +679,7 @@ void processBatch(AlignCall& call, AlignWorker& w, uint64_t begin, uint32_t nb, 
 
     // ---- compaction + output of the kept alignments ---------------------------------------------------
     exclusiveScan<uint32_t>(b.keep.get(), b.keepIndex.get(), nb, total32, w.scanWs.get(), st);
-    SHB_LAUNCH(widenBytesKernel, ceilDiv(nb, 256), 256, 0, st, (const uint32_t*)b.bytes32.get(), nb, b.bytes64.get());
+    SHB_LAUNCH(widenKernel<uint32_t>, ceilDiv(nb, 256), 256, 0, st, (const uint32_t*)b.bytes32.get(), nb, b.bytes64.get());
     exclusiveScan<unsigned long long>(b.bytes64.get(), b.bytesOff.get(), nb, total64, b.scanWs64.get(), st);
     struct { unsigned long long bytes; uint32_t kept; } totals;
     SHB_CUDA(cudaMemcpyAsync(&totals.bytes, total64, sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
@@ -786,8 +771,8 @@ void computeAlignments(shb_context* c, const void* candidatesHost, uint64_t n, c
     cudaStream_t st = c->stream;
     g_launchCount = 0;
     const auto wall0 = std::chrono::steady_clock::now();
-    Events totalEv;
-    SHB_CUDA(cudaEventRecord(totalEv.a, st));
+    EventTimer totalTimer;
+    totalTimer.start(st);
 
     AlignCall call;
     call.c = c; call.ac = &cache(c); call.o = o; call.n = n;
@@ -873,7 +858,7 @@ void computeAlignments(shb_context* c, const void* candidatesHost, uint64_t n, c
     for(uint32_t k = 0; k < workerCount; k++) ac.workers[k]->init();
     if(!ac.finalStream) SHB_CUDA(cudaStreamCreateWithFlags(&ac.finalStream, cudaStreamNonBlocking));
     call.finalStream = ac.finalStream;
-    call.digests = c->scalars.get() + 58;
+    call.digests = c->scalar(kSlotAlignmentDigests);
     SHB_CUDA(cudaMemsetAsync(call.digests, 0, 2 * sizeof(unsigned long long), st));
     // Host result blocks up front when recycled, page-locked blocks are available (every call after the first of a steady
     // caller): records and toc by their upper bound (every candidate kept), the compressed bytes by the previous call's bytes per
@@ -946,10 +931,9 @@ void computeAlignments(shb_context* c, const void* candidatesHost, uint64_t n, c
     uint64_t* tocHostOut = static_cast<uint64_t*>(tocOut.p);
     tocHostOut[count] = outBytes;
     if(count == 0) tocHostOut[0] = 0;
-    SHB_CUDA(cudaEventRecord(totalEv.b, st));
+    totalTimer.stop(st);
     SHB_CUDA(cudaStreamSynchronize(st));
-    float totalMs = 0.f;
-    SHB_CUDA(cudaEventElapsedTime(&totalMs, totalEv.a, totalEv.b));
+    const float totalMs = totalTimer.elapsedMs();
     if(getenv("SHB_TRACE")) {
         fprintf(stderr, "[shb] computeAlignments: %u worker(s), %llu batches, %llu candidates skipped as too wide for the DP kernels\n",
                 workerCount, (unsigned long long)call.ledger.size(), tooWide);
@@ -963,9 +947,8 @@ void computeAlignments(shb_context* c, const void* candidatesHost, uint64_t n, c
         result->dpMs = dpMs / double(workerCount); result->totalMs = totalMs; result->kernelLaunches = launches;
         result->alignmentDataDigest = digestHost[0]; result->compressedDigest = digestHost[1];
         result->workers = workerCount;
-        const auto wall1 = std::chrono::steady_clock::now();
-        result->outputCopyMs = std::chrono::duration<double, std::milli>(wall1 - copy0).count();
-        result->hostWallMs = std::chrono::duration<double, std::milli>(wall1 - wall0).count();
+        result->outputCopyMs = msSince(copy0);
+        result->hostWallMs = msSince(wall0);
     }
     *alignmentDataOut = recOut.take(); *alignmentCountOut = count;
     *compressedTocOut = static_cast<uint64_t*>(tocOut.take()); *compressedDataOut = static_cast<uint8_t*>(dataOut.take());

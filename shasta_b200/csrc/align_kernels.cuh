@@ -1286,12 +1286,6 @@ static __global__ void bandCellsKernel(const DpJob* __restrict__ jobs, uint32_t 
     if((threadIdx.x & 31u) == 0 && cells) atomicAdd(counter, cells);
 }
 
-static __global__ void widenBytesKernel(const uint32_t* __restrict__ in, uint32_t n, unsigned long long* __restrict__ out)
-{
-    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
-    if(p < n) out[p] = in[p];
-}
-
 } // namespace shb
 
 // =============================================================================================

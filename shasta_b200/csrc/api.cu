@@ -123,7 +123,7 @@ shb_status shb_context_create(int device, shb_context** ctx)
         SHB_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
         SHB_CUDA(cudaStreamCreateWithFlags(&c->copyStream[0], cudaStreamNonBlocking));
         SHB_CUDA(cudaStreamCreateWithFlags(&c->copyStream[1], cudaStreamNonBlocking));
-        c->scalars.reserve(512);        // never reallocated: device pointers into it are held across calls
+        c->scalars.reserve(shb::kScalarWords);     // never reallocated: device pointers into it are held across calls
         *ctx = c;
     });
 }

@@ -1,9 +1,10 @@
 // Shared host-side helpers for the CUDA library: error propagation to the C ABI, RAII device
-// buffers, launch accounting.
+// buffers, launch accounting, read-backs and timers.
 #pragma once
 
 #include <cuda_runtime.h>
 #include <algorithm>
+#include <chrono>
 #include <utility>
 #include <cstdint>
 #include <cstdio>
@@ -89,5 +90,51 @@ private:
 };
 
 inline uint32_t ceilDiv(uint64_t a, uint64_t b) { return uint32_t((a + b - 1) / b); }
+
+// Bits needed for every value in [0, maxValue]: at least 1. A sort over n rows takes bitsFor(n ? n - 1 : 0) row bits.
+inline uint32_t bitsFor(uint64_t maxValue)
+{
+    uint32_t b = 0;
+    while(b < 64 && (maxValue >> b)) b++;
+    return b ? b : 1;
+}
+
+// One value copied back from the device, with one synchronisation of the stream.
+template<class T> T readBack(const T* dev, cudaStream_t stream)
+{
+    T v;
+    SHB_CUDA(cudaMemcpyAsync(&v, dev, sizeof(T), cudaMemcpyDeviceToHost, stream));
+    SHB_CUDA(cudaStreamSynchronize(stream));
+    return v;
+}
+
+// A start and a stop timing event. elapsedMs() needs the stop event to have completed: the caller synchronises.
+struct EventTimer {
+    cudaEvent_t startEvent = nullptr, stopEvent = nullptr;
+    EventTimer()
+    {
+        SHB_CUDA(cudaEventCreate(&startEvent));
+        const cudaError_t e = cudaEventCreate(&stopEvent);
+        if(e != cudaSuccess) cudaEventDestroy(startEvent);
+        SHB_CUDA(e);
+    }
+    EventTimer(const EventTimer&) = delete;
+    EventTimer& operator=(const EventTimer&) = delete;
+    ~EventTimer() { cudaEventDestroy(startEvent); cudaEventDestroy(stopEvent); }
+    void start(cudaStream_t stream) { SHB_CUDA(cudaEventRecord(startEvent, stream)); }
+    void stop(cudaStream_t stream) { SHB_CUDA(cudaEventRecord(stopEvent, stream)); }
+    float elapsedMs() const
+    {
+        float ms = 0.f;
+        SHB_CUDA(cudaEventElapsedTime(&ms, startEvent, stopEvent));
+        return ms;
+    }
+};
+
+// Wall-clock milliseconds since t0.
+inline double msSince(std::chrono::steady_clock::time_point t0)
+{
+    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+}
 
 } // namespace shb

@@ -18,6 +18,41 @@ inline uint32_t envCount(const char* name, uint32_t dflt)
 }
 
 constexpr int kMaxFusedIterations = 16;         // LowHash iterations hashed per pass over the k-mer ids (one slab each)
+
+// The words of shb_context::scalars, the context's small device scratch for totals and counters. Every stage has slots of
+// its own, so no two stages share a word whatever the order of the calls. The uint32 totals use the low half of their word.
+enum ScalarSlot : uint32_t {
+    kSlotSweepCounts = 0,                                       // lowhash: low hashes per fused iteration
+    kSlotSegmentTotal = kSlotSweepCounts + kMaxFusedIterations, // lowhash: segments, high-frequency pairs (uint32)
+    kSlotPairCursor,                                            // lowhash: pairs written
+    kSlotPairHits,                                              // lowhash: pair hits (read with kSlotPairCursor in one copy)
+    kSlotCandidateDigest,                                       // lowhash: digest of the emitted candidates (also read by dist.cu)
+    kSlotPartitionCounts,                                       // devicePartition: one count per digit, 256 digits
+    kSlotDownsampleTotal = kSlotPartitionCounts + 256,          // align: downsampled markers of a chunk (uint32)
+    kSlotAlignmentDigests,                                      // align: AlignmentData digest, compressed alignment digest
+    kSlotMarkerTotal = kSlotAlignmentDigests + 2,               // markers: markers of strand 0
+    kSlotKeptAlignments,                                        // readgraph: alignments kept (uint32)
+    kSlotBadConnectivity,                                       // readgraph_flags: bad ReadGraphConnectivity entries (uint32)
+    kSlotMarkerGraphVertices,                                   // markergraph: errKmer, errFormat, alignedCount, maxSize, scan total, bigCount
+    kSlotMarkerGraphRcErrors = kSlotMarkerGraphVertices + 6,    // markergraph: errMarker, errVertex
+    kScalarSlotEnd = kSlotMarkerGraphRcErrors + 2
+};
+constexpr uint32_t kScalarWords = 512;                          // reserved once at context creation, never reallocated
+static_assert(kScalarSlotEnd <= kScalarWords, "the scalar slots do not fit the reserved words");
+
+// Device bytes a call holds, and their high-water mark.
+struct Footprint {
+    uint64_t live = 0, peak = 0;
+    template<class T> void add(DeviceBuffer<T>& b, uint64_t n)
+    {
+        const uint64_t before = b.capacity();
+        b.reserve(n);
+        live += (b.capacity() - before) * sizeof(T);
+        peak = std::max(peak, live);
+    }
+    template<class T> void drop(DeviceBuffer<T>& b) { live -= b.capacity() * sizeof(T); b.release(); }
+};
+
 struct LowHashAccumulator {
     uint64_t count = 0;     // reduced (pairKey, count) items in the acc ping-pong buffers
     bool inB = false;       // which of the acc ping-pong buffers holds the data
@@ -62,7 +97,8 @@ struct shb_context {
     // ---- shared workspaces --------------------------------------------------------------------
     shb::SortWorkspace sortWs;
     shb::DeviceBuffer<uint32_t> scanWs;
-    shb::DeviceBuffer<unsigned long long> scalars;   // small device scratch for totals/counters
+    shb::DeviceBuffer<unsigned long long> scalars;   // small device scratch for totals/counters: shb::ScalarSlot
+    unsigned long long* scalar(shb::ScalarSlot slot) const { return scalars.get() + slot; }
 
     // ---- LowHash buffers (see lowhash.cu) -----------------------------------------------------
     shb::DeviceBuffer<uint64_t> sweepKeys;  shb::DeviceBuffer<uint32_t> sweepVals;
@@ -86,3 +122,13 @@ struct shb_context {
     // ---- multi-GPU state (NCCL communicator, exchange buffers, gathered markers; see dist.cu) --------
     void* dist = nullptr;
 };
+
+namespace shb {
+// The stages after the alignments work on the markers of every read.
+inline void requireWholeAssembly(shb_context* c, const char* what)
+{
+    SHB_REQUIRE(c->haveMarkers, SHB_ERR_STATE, "No markers: call shb_set_markers* or shb_find_markers first.");
+    SHB_REQUIRE(c->readBegin == 0 && c->readEnd == c->readCountTotal, SHB_ERR_STATE,
+                std::string(what) + " needs the markers of every read on one context.");
+}
+}

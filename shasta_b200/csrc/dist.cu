@@ -138,12 +138,6 @@ void destroyDistState(shb_context* c)
 
 namespace {
 
-struct EventPair {
-    cudaEvent_t a = nullptr, b = nullptr;
-    EventPair() { cudaEventCreate(&a); cudaEventCreate(&b); }
-    ~EventPair() { if(a) cudaEventDestroy(a); if(b) cudaEventDestroy(b); }
-};
-
 double seconds(std::chrono::steady_clock::time_point a, std::chrono::steady_clock::time_point b)
 {
     return std::chrono::duration<double>(b - a).count();
@@ -195,13 +189,6 @@ template<class T> void exchange(DistState& d, const T* send, const uint64_t* sen
     SHB_NCCL(nccl().GroupEnd());
 }
 
-uint32_t bitsFor(uint64_t maxValue)
-{
-    uint32_t b = 0;
-    while(b < 64 && (maxValue >> b)) b++;
-    return b ? b : 1;
-}
-
 } // namespace
 
 // LowHash0 over read shards. Every rank returns the g-th contiguous block of the global candidate list.
@@ -219,8 +206,8 @@ void lowhash0Sharded(shb_context* c, const shb_lowhash_params& p, void** candida
     const uint64_t R = c->readCountTotal;
     const auto t0 = std::chrono::steady_clock::now();
     d.timing = shb_dist_timing{};
-    EventPair total;
-    SHB_CUDA(cudaEventRecord(total.a, st));
+    EventTimer total;
+    total.start(st);
 
     lowhashBegin(c, p);
     LowHashState& S = lowhashState(c);
@@ -393,16 +380,15 @@ void lowhash0Sharded(shb_context* c, const shb_lowhash_params& p, void** candida
     if(outCount) SHB_CUDA(cudaMemcpyAsync(host.p, d.candRecv.get(), outCount * 12, cudaMemcpyDeviceToHost, cs));
     if(statsOut) SHB_CUDA(cudaMemcpyAsync(statsOut, c->stats.get(), 3 * R * sizeof(uint64_t), cudaMemcpyDeviceToHost, cs));
     unsigned long long digest = 0;
-    SHB_CUDA(cudaMemcpyAsync(&digest, c->scalars.get() + 41, sizeof(digest), cudaMemcpyDeviceToHost, st));
+    SHB_CUDA(cudaMemcpyAsync(&digest, c->scalar(kSlotCandidateDigest), sizeof(digest), cudaMemcpyDeviceToHost, st));
     SHB_CUDA(cudaStreamSynchronize(cs));
-    SHB_CUDA(cudaEventRecord(total.b, st));
+    total.stop(st);
     SHB_CUDA(cudaStreamSynchronize(st));
     S.candidateDigest = digest;
     lowhashReleaseLargeScratch(c);
     d.timing.finalSeconds = seconds(tFinal, std::chrono::steady_clock::now());
     d.timing.totalSeconds = seconds(t0, std::chrono::steady_clock::now());
-    float totalMs = 0.f;
-    SHB_CUDA(cudaEventElapsedTime(&totalMs, total.a, total.b));
+    const float totalMs = total.elapsedMs();
     if(result) {
         memset(result, 0, sizeof(*result));
         result->iterations = iteration; result->log2BucketCount = S.log2BucketCount; result->lowHashCount = S.lowHashCount;

@@ -18,27 +18,6 @@ thread_local uint64_t g_launchCount = 0;
 
 namespace {
 
-struct EventTimer {
-    cudaEvent_t a = nullptr, b = nullptr;
-    EventTimer() { cudaEventCreate(&a); cudaEventCreate(&b); }
-    ~EventTimer() { if(a) cudaEventDestroy(a); if(b) cudaEventDestroy(b); }
-};
-
-uint32_t bitsFor(uint64_t maxValue)
-{
-    uint32_t b = 0;
-    while(b < 64 && (maxValue >> b)) b++;
-    return b ? b : 1;
-}
-
-template<class T> T readScalar(const T* dev, cudaStream_t stream)
-{
-    T v;
-    SHB_CUDA(cudaMemcpyAsync(&v, dev, sizeof(T), cudaMemcpyDeviceToHost, stream));
-    SHB_CUDA(cudaStreamSynchronize(stream));
-    return v;
-}
-
 // Sizes of the fused-iteration groups the default feature length (m = 4, every shipped configuration) has a fully
 // unrolled kernel for; the iteration loop of lowhash0 cuts the iterations into groups of these sizes.
 const uint32_t kUnrolledGroups[] = {16, 10, 8, 4, 2, 1};
@@ -99,13 +78,12 @@ uint32_t buildSegments(shb_context* c, const uint64_t* sortedKeys, uint32_t n, i
     c->indexBuf.reserve(n);
     c->segStartBuf.reserve(uint64_t(n) + 1);
     c->scanWs.reserve(scanWorkspaceElements(n));
-    // scalars: 512 entries, allocated once at context creation
     SHB_LAUNCH(headFlagsKernel, ceilDiv(n, 256), 256, 0, st, sortedKeys, n, shift, c->flagsBuf.get());
-    uint32_t* total = reinterpret_cast<uint32_t*>(c->scalars.get() + 32);
+    uint32_t* total = reinterpret_cast<uint32_t*>(c->scalar(kSlotSegmentTotal));
     exclusiveScan<uint32_t>(c->flagsBuf.get(), c->indexBuf.get(), n, total, c->scanWs.get(), st);
     SHB_LAUNCH(segmentStartsKernel, ceilDiv(n, 256), 256, 0, st,
                (const uint32_t*)c->flagsBuf.get(), (const uint32_t*)c->indexBuf.get(), n, c->segStartBuf.get());
-    return wantCount ? readScalar<uint32_t>(total, st) : 0u;
+    return wantCount ? readBack(total, st) : 0u;
 }
 
 using Accumulator = LowHashAccumulator;
@@ -187,12 +165,11 @@ uint64_t countHighFrequency(shb_context* c, const Accumulator& acc, uint64_t min
     c->flagsBuf.reserve(n);
     c->indexBuf.reserve(n);
     c->scanWs.reserve(scanWorkspaceElements(n));
-    // scalars: 512 entries, allocated once at context creation
     SHB_LAUNCH(frequencyFlagsKernel, ceilDiv(n, 256), 256, 0, st, (const uint32_t*)accVals(c, acc), n, minFrequency, c->flagsBuf.get());
-    uint32_t* total = reinterpret_cast<uint32_t*>(c->scalars.get() + 32);
+    uint32_t* total = reinterpret_cast<uint32_t*>(c->scalar(kSlotSegmentTotal));
     exclusiveScan<uint32_t>(c->flagsBuf.get(), c->indexBuf.get(), n, total, c->scanWs.get(), st);
     (void)keepOffsets;
-    return readScalar<uint32_t>(total, st);
+    return readBack(total, st);
 }
 
 } // namespace
@@ -260,7 +237,6 @@ void lowhashBegin(shb_context* c, const shb_lowhash_params& p)
     if(S.capacity > M + 1) S.capacity = M + 1;
     c->stats.reserve(3 * R + 1);
     SHB_CUDA(cudaMemsetAsync(c->stats.get(), 0, (3 * R + 1) * sizeof(unsigned long long), st));
-    // scalars: 512 entries, allocated once at context creation
     S.active = true;
 }
 
@@ -278,7 +254,7 @@ void lowhashSweep(shb_context* c, uint64_t iterationBegin, uint32_t group, unsig
     for(;;) {
         c->sweepKeys.reserve(S.capacity * group);
         c->sweepVals.reserve(S.capacity * group);
-        SHB_CUDA(cudaMemsetAsync(c->scalars.get(), 0, kMaxFusedIterations * sizeof(unsigned long long), st));
+        SHB_CUDA(cudaMemsetAsync(c->scalar(kSlotSweepCounts), 0, kMaxFusedIterations * sizeof(unsigned long long), st));
         SweepArgs a;
         a.kmerIds = c->kmerIds;
         a.markerCount = M;
@@ -295,7 +271,7 @@ void lowhashSweep(shb_context* c, uint64_t iterationBegin, uint32_t group, unsig
         a.keys = c->sweepKeys.get();
         a.vals = c->sweepVals.get();
         a.capacity = S.capacity;
-        a.counts = c->scalars.get();
+        a.counts = c->scalar(kSlotSweepCounts);
         {
             const double expected = double(kSweepTile) * double(group) * S.p.hashFraction;
             a.queueCapacity = uint32_t(std::min<double>(kSweepQueueMax, std::max<double>(kSweepQueueMin, 1.5 * expected + 64.)));
@@ -311,18 +287,14 @@ void lowhashSweep(shb_context* c, uint64_t iterationBegin, uint32_t group, unsig
         a.tileFirstRead = c->sweepTileFirstRead.get();
         const bool run = M >= S.p.m && M > 0;
         if(run) {
-            SHB_CUDA(cudaEventRecord(sweepTimer.a, st));
+            sweepTimer.start(st);
             launchSweep(a, ceilDiv(ceilDiv(M, kSweepTile), uint64_t(kSweepTilesPerBlock)), st);
-            SHB_CUDA(cudaEventRecord(sweepTimer.b, st));
+            sweepTimer.stop(st);
             S.sweepLaunches++;
         }
-        SHB_CUDA(cudaMemcpyAsync(counts, c->scalars.get(), group * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+        SHB_CUDA(cudaMemcpyAsync(counts, c->scalar(kSlotSweepCounts), group * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
         SHB_CUDA(cudaStreamSynchronize(st));
-        if(run) {
-            float ms = 0.f;
-            SHB_CUDA(cudaEventElapsedTime(&ms, sweepTimer.a, sweepTimer.b));
-            S.sweepMs += ms;
-        }
+        if(run) S.sweepMs += sweepTimer.elapsedMs();
         const unsigned long long worst = *std::max_element(counts, counts + group);
         if(worst <= S.capacity) break;
         S.capacity = worst + worst / 8 + 1024;        // slab overflow: grow and redo this group
@@ -367,8 +339,8 @@ void lowhashProcessEntries(shb_context* c, uint64_t* keysA, uint32_t* valsA, uin
         const uint64_t* sortedReadKeys = flipped ? c->pairsB.get() : otherKeys;
         const uint32_t* order = flipped ? c->countsBuf.get() : otherVals;
         const uint32_t numReads = buildSegments(c, sortedReadKeys, n, 0);
-        unsigned long long* cursor = c->scalars.get() + 40;
-        unsigned long long* hits = c->scalars.get() + 43;
+        unsigned long long* cursor = c->scalar(kSlotPairCursor);
+        unsigned long long* hits = c->scalar(kSlotPairHits);
         uint32_t maxProbes = kPairTableMaxProbes;
         if(const char* e = std::getenv("SHB_LOWHASH_TABLE_PROBES")) maxProbes = uint32_t(std::max(1, std::atoi(e)));     // test hook: force the overflow path
         for(;;) {
@@ -380,13 +352,14 @@ void lowhashProcessEntries(shb_context* c, uint64_t* keysA, uint32_t* valsA, uin
             SHB_LAUNCH(readPairsKernel, ceilDiv(numReads, kPairTableWarps), kPairTableWarps * 32, 0, st, keys, vals, (const uint2*)span,
                        sortedReadKeys, order, (const uint32_t*)c->segStartBuf.get(), numReads, cursor, hits,
                        accKeys(c, S.acc) + S.acc.count, accVals(c, S.acc) + S.acc.count, (unsigned long long)room, maxProbes);
-            unsigned long long totals[4];      // scalars 40..43: cursor, (candidate digest), (marker total), hits
-            SHB_CUDA(cudaMemcpyAsync(totals, cursor, 4 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+            static_assert(kSlotPairHits == kSlotPairCursor + 1, "cursor and hits are read in one copy");
+            unsigned long long totals[2];      // cursor, hits
+            SHB_CUDA(cudaMemcpyAsync(totals, cursor, sizeof(totals), cudaMemcpyDeviceToHost, st));
             SHB_CUDA(cudaStreamSynchronize(st));
             if(totals[0] <= room) {
                 S.acc.count += totals[0];
                 if(totals[0]) S.acc.sorted = false;
-                S.pairCount += totals[3];
+                S.pairCount += totals[1];
                 break;
             }
             accReserve(c, S.acc, S.acc.count + totals[0] + totals[0] / 16);
@@ -398,7 +371,7 @@ void lowhashProcessEntries(shb_context* c, uint64_t* keysA, uint32_t* valsA, uin
     // One pass: per-read statistics and the pair hits, appended (in any order) to the raw pair buffer; sorting and counting
     // happen once for many iterations. The pass reports the exact number of hits; if they did not fit, the buffer grows
     // (after a reduction of what it holds, when that would exceed the limit) and the pass runs again without the statistics.
-    unsigned long long* cursor = c->scalars.get() + 40;
+    unsigned long long* cursor = c->scalar(kSlotPairCursor);
     if(c->pairsA.capacity() == 0) c->pairsA.reserve(1ull << 20);
     bool withStats = true;
     for(;;) {
@@ -407,7 +380,7 @@ void lowhashProcessEntries(shb_context* c, uint64_t* keysA, uint32_t* valsA, uin
         SHB_LAUNCH(bucketPairsKernel, ceilDiv(n, 256), 256, 0, st, keys, vals, n, p.minBucketSize, p.maxBucketSize,
                    withStats ? c->stats.get() : (unsigned long long*)nullptr, cursor, c->pairsA.get() + S.acc.rawCount,
                    (unsigned long long)room);
-        const unsigned long long np64 = readScalar<unsigned long long>(cursor, st);
+        const unsigned long long np64 = readBack(cursor, st);
         SHB_REQUIRE(np64 < (1ull << 32), SHB_ERR_INVALID,
                     "LowHash0: more than 2^32-1 candidate pair hits in one iteration (maxBucketSize too large).");
         if(np64 <= room) {
@@ -456,7 +429,7 @@ void lowhashSetPairs(shb_context* c, const uint64_t* keys, const uint32_t* count
 }
 
 // Final merge + emission, src/LowHash0.cpp:204-214, left on the device: c->candidatesDev holds nOut 12-byte records.
-// The digest of the emitted records is computed asynchronously into S.candidateDigest's device slot (scalars[41]).
+// The digest of the emitted records is computed asynchronously into S.candidateDigest's device slot (kSlotCandidateDigest).
 uint64_t lowhashEmitDevice(shb_context* c)
 {
     LowHashState& S = lowhashState(c);
@@ -466,7 +439,7 @@ uint64_t lowhashEmitDevice(shb_context* c)
     reduceRawPairs(c, S.acc, S.readBits);
     mergeAccumulator(c, S.acc, S.readBits);
     const uint64_t nOut = countHighFrequency(c, S.acc, S.p.minFrequency, true);
-    unsigned long long* digestDev = c->scalars.get() + 41;
+    unsigned long long* digestDev = c->scalar(kSlotCandidateDigest);
     SHB_CUDA(cudaMemsetAsync(digestDev, 0, sizeof(unsigned long long), st));
     if(nOut) {
         c->candidatesDev.reserve(3 * nOut);
@@ -511,7 +484,7 @@ void lowhashEmit(shb_context* c, void** candidatesOut, uint64_t* candidateCountO
     SHB_REQUIRE(host.p != nullptr, SHB_ERR_OOM, "Out of host memory for the alignment candidates.");
     unsigned long long digest = 0;
     if(nOut) SHB_CUDA(cudaMemcpyAsync(host.p, c->candidatesDev.get(), nOut * 12, cudaMemcpyDeviceToHost, st));
-    SHB_CUDA(cudaMemcpyAsync(&digest, c->scalars.get() + 41, sizeof(digest), cudaMemcpyDeviceToHost, st));
+    SHB_CUDA(cudaMemcpyAsync(&digest, c->scalar(kSlotCandidateDigest), sizeof(digest), cudaMemcpyDeviceToHost, st));
     SHB_CUDA(cudaStreamSynchronize(st));
     S.candidateDigest = digest;
     *candidatesOut = host.take();
@@ -540,8 +513,7 @@ void devicePartition(shb_context* c, uint64_t* keys, uint32_t* vals, uint64_t n,
     const bool inB = radixSort<true>(keys, c->partKeys.get(), vals, c->partVals.get(), n, range, 1, c->sortWs, st);
     uint64_t* sortedKeys = inB ? c->partKeys.get() : keys;
     // Digit boundaries by binary search on the host-visible sorted keys would need a copy; count on the device instead.
-    // scalars: 512 entries, allocated once at context creation
-    unsigned long long* dCounts = c->scalars.get() + 64;
+    unsigned long long* dCounts = c->scalar(kSlotPartitionCounts);
     SHB_CUDA(cudaMemsetAsync(dCounts, 0, buckets * sizeof(unsigned long long), st));
     SHB_LAUNCH(digitCountKernel, ceilDiv(n, 256), 256, 0, st, (const uint64_t*)sortedKeys, uint32_t(n), int(shift), buckets - 1u, dCounts);
     std::vector<unsigned long long> h(buckets);
@@ -572,7 +544,7 @@ void lowhash0(shb_context* c, const shb_lowhash_params& p,
     LowHashState& S = lowhashState(c);
     cudaStream_t st = c->stream;
     EventTimer totalTimer;
-    SHB_CUDA(cudaEventRecord(totalTimer.a, st));
+    totalTimer.start(st);
     const bool perIteration = (p.perIterationMerge != 0) || (p.minHashIterationCount == 0);
 
     uint64_t highFrequency = 0;
@@ -610,10 +582,9 @@ void lowhash0(shb_context* c, const shb_lowhash_params& p,
     if(statsOut) {
         SHB_CUDA(cudaMemcpyAsync(statsOut, c->stats.get(), 3 * R * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
     }
-    SHB_CUDA(cudaEventRecord(totalTimer.b, st));
+    totalTimer.stop(st);
     SHB_CUDA(cudaStreamSynchronize(st));
-    float totalMs = 0.f;
-    SHB_CUDA(cudaEventElapsedTime(&totalMs, totalTimer.a, totalTimer.b));
+    const float totalMs = totalTimer.elapsedMs();
     lowhashReleaseLargeScratch(c);
     if(result) {
         result->iterations = iteration;

@@ -461,26 +461,6 @@ unsigned gridFor(uint64_t n, uint32_t threads = kMgThreads)
     return unsigned(std::min<uint64_t>((n + threads - 1) / threads, 132ull * 16));
 }
 
-void requireWholeAssembly(shb_context* c, const char* what)
-{
-    SHB_REQUIRE(c->haveMarkers, SHB_ERR_STATE, "No markers: call shb_set_markers* or shb_find_markers first.");
-    SHB_REQUIRE(c->readBegin == 0 && c->readEnd == c->readCountTotal, SHB_ERR_STATE,
-                std::string(what) + " needs the markers of every read on one context.");
-}
-
-struct HostBlocks4 {        // frees what was not handed to the caller (error paths)
-    void* p[4] = {nullptr, nullptr, nullptr, nullptr};
-    ~HostBlocks4() { for(void* q : p) if(q) HostPool::instance().release(q); }
-    void disarm() { for(void*& q : p) q = nullptr; }
-};
-
-// Device bytes this call holds, and their high-water mark.
-struct Footprint {
-    uint64_t live = 0, peak = 0;
-    template<class T> void add(DeviceBuffer<T>& b, uint64_t n) { const uint64_t before = b.capacity(); b.reserve(n); live += (b.capacity() - before) * sizeof(T); peak = std::max(peak, live); }
-    template<class T> void drop(DeviceBuffer<T>& b) { live -= b.capacity() * sizeof(T); b.release(); }
-};
-
 } // namespace
 
 // PeakFinder::findPeaks + findXCutoff (src/PeakFinder.cpp:23-198). Returns true where the reference throws
@@ -596,14 +576,12 @@ void createMarkerGraphVertices(shb_context* c, const shb_marker_graph_params& p,
     Footprint fp;
     DeviceBuffer<uint64_t> P;
     fp.add(P, M + 1);
-    cudaEvent_t ev[2];
-    SHB_CUDA(cudaEventCreate(&ev[0])); SHB_CUDA(cudaEventCreate(&ev[1]));
-    struct EventGuard { cudaEvent_t* e; ~EventGuard() { cudaEventDestroy(e[0]); cudaEventDestroy(e[1]); } } eventGuard{ev};
-    SHB_CUDA(cudaEventRecord(ev[0], st));
+    EventTimer timer;
+    timer.start(st);
     if(M) SHB_LAUNCH(initParentKernel, gridFor(M), kMgThreads, 0, st, P.get(), M);
 
     // Union, in batches of edge pairs (SHB_MARKERGRAPH_PAIR_BATCH, SHB_MARKERGRAPH_BATCH_BYTES: test hooks).
-    unsigned long long* scal = c->scalars.get() + 128;    // errKmer, errFormat, alignedCount, maxSize, scan total, bigCount
+    unsigned long long* scal = c->scalar(kSlotMarkerGraphVertices);    // errKmer, errFormat, alignedCount, maxSize, scan total, bigCount
     const unsigned long long init[6] = {~0ull, ~0ull, 0, 0, 0, 0};
     SHB_CUDA(cudaMemcpyAsync(scal, init, sizeof(init), cudaMemcpyHostToDevice, st));
     {
@@ -659,13 +637,11 @@ void createMarkerGraphVertices(shb_context* c, const shb_marker_graph_params& p,
         SHB_LAUNCH(countKernel, gridFor(M), kMgThreads, 0, st, P.get(), M);
         SHB_LAUNCH(histogramKernel, gridFor(M), kMgThreads, 0, st, (const uint64_t*)P.get(), M, (unsigned long long*)nullptr, scal + 3);
     }
-    uint64_t maxSize = 0;
-    SHB_CUDA(cudaMemcpyAsync(&maxSize, scal + 3, 8, cudaMemcpyDeviceToHost, st));
-    SHB_CUDA(cudaStreamSynchronize(st));
+    const uint64_t maxSize = readBack(scal + 3, st);
     const uint64_t histSize = M ? maxSize + 1 : 0;
-    HostBlocks4 hb;
-    uint64_t* hist = (uint64_t*)(hb.p[3] = allocHostResult(8 * histSize + 8));
-    SHB_REQUIRE(hist, SHB_ERR_OOM, "Out of host memory for the histogram.");
+    HostResult histBlock(allocHostResult(8 * histSize + 8));
+    SHB_REQUIRE(histBlock.p, SHB_ERR_OOM, "Out of host memory for the histogram.");
+    uint64_t* hist = static_cast<uint64_t*>(histBlock.p);
     if(M) {
         DeviceBuffer<unsigned long long> dHist;
         fp.add(dHist, histSize);
@@ -704,8 +680,7 @@ void createMarkerGraphVertices(shb_context* c, const shb_marker_graph_params& p,
         fp.add(tileOffsets, tiles + 1); fp.add(scanWs, scanWorkspaceElements(tiles) + 1);
         SHB_LAUNCH(keptTileCountKernel, unsigned(tiles), kScanThreads, 0, st, (const uint64_t*)P.get(), M, minCoverage, p.maxCoverage, tileOffsets.get());
         exclusiveScan<uint64_t>(tileOffsets.get(), tileOffsets.get(), tiles, total, scanWs.get(), st);
-        SHB_CUDA(cudaMemcpyAsync(&keptSets, total, 8, cudaMemcpyDeviceToHost, st));
-        SHB_CUDA(cudaStreamSynchronize(st));
+        keptSets = readBack(total, st);
         fp.add(setSize, keptSets + 1);
         SHB_LAUNCH(keptTileWriteKernel, unsigned(tiles), kScanThreads, 0, st, P.get(), M, minCoverage, p.maxCoverage,
                    (const uint64_t*)tileOffsets.get(), setSize.get());
@@ -721,10 +696,9 @@ void createMarkerGraphVertices(shb_context* c, const shb_marker_graph_params& p,
     if(keptSets) {
         fp.add(setOffset, keptSets + 1); fp.add(scanWs, scanWorkspaceElements(keptSets) + 1);
         exclusiveScan<uint64_t>(setSize.get(), setOffset.get(), keptSets, total, scanWs.get(), st);
-        SHB_CUDA(cudaMemcpyAsync(&keptMarkers, total, 8, cudaMemcpyDeviceToHost, st));
+        keptMarkers = readBack(total, st);
         fp.add(cursor, keptSets);
         SHB_CUDA(cudaMemsetAsync(cursor.get(), 0, 4 * keptSets, st));
-        SHB_CUDA(cudaStreamSynchronize(st));
         fp.add(keys, keptMarkers + 1);
         SHB_LAUNCH(scatterKernel, ceilDiv(uint64_t(rows) * 32, kMgThreads), kMgThreads, 0, st, (const uint64_t*)P.get(),
                    (const uint64_t*)c->toc.get(), rows, (const uint64_t*)setOffset.get(), cursor.get(), keys.get());
@@ -732,9 +706,7 @@ void createMarkerGraphVertices(shb_context* c, const shb_marker_graph_params& p,
         fp.add(bigSets, keptSets);
         SHB_LAUNCH(warpSortKernel, ceilDiv(keptSets * 32, kMgThreads), kMgThreads, 0, st, keys.get(), (const uint64_t*)setOffset.get(),
                    (const uint64_t*)setSize.get(), keptSets, bigSets.get(), scal + 5);
-        uint64_t bigCount = 0;
-        SHB_CUDA(cudaMemcpyAsync(&bigCount, scal + 5, 8, cudaMemcpyDeviceToHost, st));
-        SHB_CUDA(cudaStreamSynchronize(st));
+        const uint64_t bigCount = readBack(scal + 5, st);
         if(bigCount) {
             // The listed sets in a fixed order (the list's order comes from atomics), split by size.
             std::vector<uint64_t> big(bigCount), sizes(keptSets), offsets(keptSets);
@@ -793,16 +765,17 @@ void createMarkerGraphVertices(shb_context* c, const shb_marker_graph_params& p,
     res.badDisjointSetCount = keptSets - V;
 
     // Host outputs: MarkerGraphVertexTable (Uint40 per marker), MarkerGraphVertices toc (Uint40) and data (uint64).
-    uint8_t* table = (uint8_t*)(hb.p[0] = allocHostResult(5 * M + 8));
-    uint8_t* toc5 = (uint8_t*)(hb.p[1] = allocHostResult(5 * (V + 1) + 8));
-    uint64_t* vdata = (uint64_t*)(hb.p[2] = allocHostResult(8 * vertexMarkers + 8));
-    SHB_REQUIRE(table && toc5 && vdata, SHB_ERR_OOM, "Out of host memory for the marker graph vertices.");
+    HostResult tableBlock(allocHostResult(5 * M + 8)), toc5Block(allocHostResult(5 * (V + 1) + 8)),
+               vdataBlock(allocHostResult(8 * vertexMarkers + 8));
+    SHB_REQUIRE(tableBlock.p && toc5Block.p && vdataBlock.p, SHB_ERR_OOM, "Out of host memory for the marker graph vertices.");
+    uint8_t* table = static_cast<uint8_t*>(tableBlock.p);
+    uint8_t* toc5 = static_cast<uint8_t*>(toc5Block.p);
     DeviceBuffer<uint8_t> stage;
     if(V) {
         fp.add(stage, 5 * (V + 1));
         SHB_LAUNCH(toc40Kernel, gridFor(V + 1), kMgThreads, 0, st, (const uint64_t*)vtoc.get(), V + 1, stage.get());
         SHB_CUDA(cudaMemcpyAsync(toc5, stage.get(), 5 * (V + 1), cudaMemcpyDeviceToHost, st));
-        SHB_CUDA(cudaMemcpyAsync(vdata, data.get(), 8 * vertexMarkers, cudaMemcpyDeviceToHost, st));
+        SHB_CUDA(cudaMemcpyAsync(vdataBlock.p, data.get(), 8 * vertexMarkers, cudaMemcpyDeviceToHost, st));
         SHB_CUDA(cudaStreamSynchronize(st));
     } else {
         memset(toc5, 0, 5);
@@ -821,18 +794,17 @@ void createMarkerGraphVertices(shb_context* c, const shb_marker_graph_params& p,
             SHB_CUDA(cudaStreamSynchronize(st));
         }
     }
-    SHB_CUDA(cudaEventRecord(ev[1], st));
-    SHB_CUDA(cudaEventSynchronize(ev[1]));
-    float ms = 0;
-    SHB_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+    timer.stop(st);
+    SHB_CUDA(cudaEventSynchronize(timer.stopEvent));
+    const float ms = timer.elapsedMs();
 
-    *vertexTableOut = table; *verticesTocOut = toc5; *verticesDataOut = vdata; *histogramOut = hist;
-    hb.disarm();
+    *vertexTableOut = static_cast<uint8_t*>(tableBlock.take()); *verticesTocOut = static_cast<uint8_t*>(toc5Block.take());
+    *verticesDataOut = static_cast<uint64_t*>(vdataBlock.take()); *histogramOut = static_cast<uint64_t*>(histBlock.take());
     if(result) {
         res.histogramSize = histSize;
         res.peakDeviceBytes = fp.peak;
         res.deviceMs = ms;
-        res.totalMs = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+        res.totalMs = msSince(t0);
         res.kernelLaunches = g_launchCount - launches0;
         *result = res;
     }
@@ -867,7 +839,7 @@ void findMarkerGraphReverseComplementVertices(shb_context* c, const uint8_t* tab
         SHB_CUDA(cudaMemcpyAsync(dTable.get(), table5, 5 * M, cudaMemcpyHostToDevice, st));
         SHB_CUDA(cudaMemcpyAsync(dToc.get(), vtoc.data(), 8 * (V + 1), cudaMemcpyHostToDevice, st));
         SHB_CUDA(cudaMemcpyAsync(dData.get(), vdata, 8 * n, cudaMemcpyHostToDevice, st));
-        unsigned long long* err = c->scalars.get() + 144;
+        unsigned long long* err = c->scalar(kSlotMarkerGraphRcErrors);
         const unsigned long long init[2] = {~0ull, ~0ull};
         SHB_CUDA(cudaMemcpyAsync(err, init, sizeof(init), cudaMemcpyHostToDevice, st));
         SHB_LAUNCH(rcVertexKernel, gridFor(V), kMgThreads, 0, st, (const uint8_t*)dTable.get(), (const uint64_t*)dToc.get(),

@@ -130,12 +130,6 @@ __global__ void markerWriteKernel(MarkerArgs a, const unsigned long long* __rest
     }
 }
 
-__global__ void widenCountsKernel(const uint32_t* __restrict__ in, uint64_t n, unsigned long long* __restrict__ out)
-{
-    const uint64_t i = uint64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-    if(i < n) out[i] = in[i];
-}
-
 } // namespace
 
 // The markers of reads [0, readCount) become the context's resident marker set (as after shb_set_markers with all reads on
@@ -158,9 +152,8 @@ void findMarkers(shb_context* c, uint32_t k, uint64_t readCount, const uint64_t*
         SHB_REQUIRE(baseCounts[r] < (1ull << 24), SHB_ERR_INVALID, "A read has 2^24 or more bases (marker positions are 24 bits, src/Marker.hpp:62-64).");
     }
     const uint64_t blockCount = wordCount / 2;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    SHB_CUDA(cudaEventCreate(&e0)); SHB_CUDA(cudaEventCreate(&e1));
-    SHB_CUDA(cudaEventRecord(e0, st));
+    EventTimer timer;
+    timer.start(st);
 
     // isMarker bitmap: 4^k bits
     const uint64_t kmerCount = 1ull << (2 * k);
@@ -185,16 +178,14 @@ void findMarkers(shb_context* c, uint32_t k, uint64_t readCount, const uint64_t*
     MarkerArgs a;
     a.words = dWords.get(); a.wordOffsets = dOffsets.get(); a.baseCounts = dBaseCounts.get(); a.isMarkerBits = dBitmap.get();
     a.readCount = uint32_t(readCount); a.k = k; a.blockCount = blockCount;
-    unsigned long long totalOneStrand = 0;
-    unsigned long long* totalDev = c->scalars.get() + 42;
+    unsigned long long* totalDev = c->scalar(kSlotMarkerTotal);
     SHB_CUDA(cudaMemsetAsync(totalDev, 0, sizeof(unsigned long long), st));
     if(blockCount) {
         SHB_LAUNCH(markerMaskKernel, ceilDiv(blockCount, 128), 128, 0, st, a, dMasks.get(), dCounts.get());
-        SHB_LAUNCH(widenCountsKernel, ceilDiv(blockCount, 256), 256, 0, st, (const uint32_t*)dCounts.get(), blockCount, dCounts64.get());
+        SHB_LAUNCH(widenKernel<uint64_t>, ceilDiv(blockCount, 256), 256, 0, st, (const uint32_t*)dCounts.get(), blockCount, dCounts64.get());
         exclusiveScan<unsigned long long>(dCounts64.get(), dBefore.get(), blockCount, totalDev, dScanWs.get(), st);
     }
-    SHB_CUDA(cudaMemcpyAsync(&totalOneStrand, totalDev, sizeof(totalOneStrand), cudaMemcpyDeviceToHost, st));
-    SHB_CUDA(cudaStreamSynchronize(st));
+    const unsigned long long totalOneStrand = readBack(totalDev, st);
     const uint64_t M = 2 * totalOneStrand;
 
     c->haveMarkers = false;
@@ -231,13 +222,11 @@ void findMarkers(shb_context* c, uint32_t k, uint64_t readCount, const uint64_t*
     c->readFlags.reserve(readCount + 1);
     SHB_CUDA(cudaMemcpyAsync(c->toc.get(), toc.data(), (2 * readCount + 1) * 8, cudaMemcpyHostToDevice, st));
     if(readCount) SHB_CUDA(cudaMemcpyAsync(c->readFlags.get(), readFlags, readCount, cudaMemcpyHostToDevice, st));
-    SHB_CUDA(cudaEventRecord(e1, st));
+    timer.stop(st);
     SHB_CUDA(cudaStreamSynchronize(st));
     c->kmerIds = c->kmerIdsOwned.get();
     c->haveMarkers = true;
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, e0, e1);
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
+    const float ms = timer.elapsedMs();
     if(result) {
         result->readCount = readCount; result->baseCount = 0;
         for(uint64_t r = 0; r < readCount; r++) result->baseCount += baseCounts[r];

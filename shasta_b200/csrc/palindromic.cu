@@ -367,20 +367,13 @@ void runExact(shb_context* c, const shb_palindromic_params& p, const std::vector
     }
 }
 
-void requireWholeAssembly(shb_context* c)
-{
-    SHB_REQUIRE(c->haveMarkers, SHB_ERR_STATE, "No markers: call shb_set_markers* or shb_find_markers first.");
-    SHB_REQUIRE(c->readBegin == 0 && c->readEnd == c->readCountTotal, SHB_ERR_STATE,
-                "flagPalindromicReads needs the markers of every read on one context.");
-}
-
 } // namespace
 
 void flagPalindromicReads(shb_context* c, const shb_palindromic_params& p, uint8_t* flagsOut, uint32_t* alignedOut,
                           uint32_t* nearOut, shb_palindromic_result* result)
 {
     SHB_CUDA(cudaSetDevice(c->device));
-    requireWholeAssembly(c);
+    requireWholeAssembly(c, "flagPalindromicReads");
     const uint64_t launches0 = g_launchCount;
     const auto t0 = std::chrono::steady_clock::now();
     cudaStream_t st = c->stream;
@@ -407,8 +400,7 @@ void flagPalindromicReads(shb_context* c, const shb_palindromic_params& p, uint8
             keysA.reserve(n); keysB.reserve(n); valsA.reserve(n); valsB.reserve(n);
             SHB_LAUNCH(palKeysKernel, ceilDiv(n, 256), 256, 0, st, c->kmerIds, (const uint64_t*)c->toc.get(), rowBegin, rowEnd,
                        markerBegin, n, keysA.get(), valsA.get());
-            uint32_t rowBits = 1;
-            while((1ull << rowBits) < uint64_t(rowEnd - rowBegin)) rowBits++;
+            const uint32_t rowBits = bitsFor(rowEnd - rowBegin - 1);
             const int ranges[2][2] = {{0, 32}, {32, 32 + int(rowBits)}};
             const bool inB = radixSort<true>(keysA.get(), keysB.get(), valsA.get(), valsB.get(), n, ranges, 2, c->sortWs, st);
             keys = inB ? keysB.get() : keysA.get();
@@ -436,7 +428,7 @@ void flagPalindromicReads(shb_context* c, const shb_palindromic_params& p, uint8
     std::vector<PalJob> jobs;
     ExactTotals totals;
     runExact(c, p, exactReads, jobs, nullptr, totals);
-    const auto t2 = std::chrono::steady_clock::now();
+    const double totalMs = msSince(t0), exactMs = msSince(t1);
 
     // Bit 0 of the flags: reset everywhere (src/AssemblerAlign.cpp:676-681), set on the reads phase B flags. Bits 1-7 are kept.
     uint64_t palindromic = 0;
@@ -462,8 +454,8 @@ void flagPalindromicReads(shb_context* c, const shb_palindromic_params& p, uint8
         result->edgeCount = totals.edges;
         result->heapPushCount = totals.heapPushes;
         result->heapsortFallbackCount = totals.fallbacks;
-        result->totalMs = std::chrono::duration<double, std::milli>(t2 - t0).count();
-        result->exactMs = std::chrono::duration<double, std::milli>(t2 - t1).count();
+        result->totalMs = totalMs;
+        result->exactMs = exactMs;
         result->kernelLaunches = g_launchCount - launches0;
     }
 }
@@ -471,7 +463,7 @@ void flagPalindromicReads(shb_context* c, const shb_palindromic_params& p, uint8
 void palindromicReadAlignment(shb_context* c, uint64_t readId, const shb_palindromic_params& p, uint32_t** ordinals, uint64_t* count)
 {
     SHB_CUDA(cudaSetDevice(c->device));
-    requireWholeAssembly(c);
+    requireWholeAssembly(c, "flagPalindromicReads");
     SHB_REQUIRE(readId < c->readCountTotal, SHB_ERR_INVALID, "Read id out of range.");
     std::vector<PalJob> jobs;
     std::vector<std::vector<uint32_t>> paths;

@@ -144,4 +144,22 @@ static __global__ void segmentStartsKernel(const uint32_t* __restrict__ flags, c
     if(i == n - 1) segStart[segIndexExclusive[i] + flags[i]] = n;
 }
 
+// Row starts of a table sorted by row (bits 32-63 of the keys): toc[row] = the first of `entries` keys whose row is >= row,
+// for row = 0 ... rows.
+template<class T> __global__ void rowStartsKernel(const uint64_t* __restrict__ sortedKeys, uint32_t entries, uint32_t rows, T* __restrict__ toc)
+{
+    const uint32_t row = blockIdx.x * blockDim.x + threadIdx.x;
+    if(row > rows) return;
+    uint32_t lo = 0, hi = entries;
+    while(lo < hi) { const uint32_t mid = lo + ((hi - lo) >> 1); if(uint32_t(sortedKeys[mid] >> 32) < row) lo = mid + 1; else hi = mid; }
+    toc[row] = T(lo);
+}
+
+// out[i] = in[i] widened to 64 bits, for i < n. N, the index type, is uint32_t or uint64_t.
+template<class N> __global__ void widenKernel(const uint32_t* __restrict__ in, N n, unsigned long long* __restrict__ out)
+{
+    const N i = N(blockIdx.x) * blockDim.x + threadIdx.x;
+    if(i < n) out[i] = in[i];
+}
+
 } // namespace shb

@@ -81,21 +81,6 @@ __global__ void readGraphEdgesKernel(const uint32_t* __restrict__ records, uint3
     }
 }
 
-__global__ void readGraphTocKernel(const uint64_t* __restrict__ sortedKeys, uint32_t entries, uint32_t rows, uint32_t* __restrict__ toc)
-{
-    const uint32_t row = blockIdx.x * blockDim.x + threadIdx.x;
-    if(row > rows) return;
-    uint32_t lo = 0, hi = entries;                      // first entry whose row is >= this row
-    while(lo < hi) { const uint32_t mid = lo + ((hi - lo) >> 1); if(uint32_t(sortedKeys[mid] >> 32) < row) lo = mid + 1; else hi = mid; }
-    toc[row] = lo;
-}
-
-struct HostBlocks {         // frees what was not handed to the caller (error paths)
-    void* p[4] = {nullptr, nullptr, nullptr, nullptr};
-    ~HostBlocks() { for(void* q : p) if(q) HostPool::instance().release(q); }
-    void disarm() { for(void*& q : p) q = nullptr; }
-};
-
 // shasta::Histogram2 (src/Histogram.cpp:14-140) as createReadGraph2 uses it: dynamicBounds = true. update() grows the
 // histogram to `index` bins when index > size and then increments bin `index` — which, for index >= the size before the call,
 // lies one past the end: the reference's write lands outside the deque and the sample is never seen by getSum() /
@@ -181,10 +166,10 @@ void createReadGraph(shb_context* c, void* alignmentData, uint64_t n, uint64_t r
     cudaStream_t st = c->stream;
     uint32_t* rec = static_cast<uint32_t*>(alignmentData);
     const uint32_t rows = uint32_t(2 * readCount);
-    HostBlocks hb;
-    uint8_t* keepHost = (uint8_t*)(hb.p[0] = allocHostResult(n + 1));
-    uint32_t* toc = (uint32_t*)(hb.p[1] = allocHostResult(4ull * (uint64_t(rows) + 1)));
-    SHB_REQUIRE(keepHost && toc, SHB_ERR_OOM, "Out of host memory for the read graph.");
+    HostResult keepBlock(allocHostResult(n + 1)), tocBlock(allocHostResult(4ull * (uint64_t(rows) + 1)));
+    SHB_REQUIRE(keepBlock.p && tocBlock.p, SHB_ERR_OOM, "Out of host memory for the read graph.");
+    uint8_t* keepHost = static_cast<uint8_t*>(keepBlock.p);
+    uint32_t* toc = static_cast<uint32_t*>(tocBlock.p);
     for(uint64_t i = 0; i < n; i++) {
         SHB_REQUIRE(rec[kAlignmentWords * i] < readCount && rec[kAlignmentWords * i + 1] < readCount, SHB_ERR_INVALID,
                     "One of the alignments refers to a read that does not exist.");
@@ -212,16 +197,12 @@ void createReadGraph(shb_context* c, void* alignmentData, uint64_t n, uint64_t r
             SHB_LAUNCH(readGraphKeepKernel, ceilDiv(items, 256), 256, 0, st, (const uint64_t*)(inB ? keysB.get() : keysA.get()),
                        (const uint32_t*)(inB ? valsB.get() : valsA.get()), items, maxAlignmentCount, keep.get());
         }
-        uint32_t* totalDev = reinterpret_cast<uint32_t*>(c->scalars.get() + 32);
+        uint32_t* totalDev = reinterpret_cast<uint32_t*>(c->scalar(kSlotKeptAlignments));
         exclusiveScan<uint32_t>(keep.get(), keepIndex.get(), n, totalDev, scanWs.get(), st);
-        uint32_t kept = 0;
-        SHB_CUDA(cudaMemcpyAsync(&kept, totalDev, sizeof(kept), cudaMemcpyDeviceToHost, st));
-        SHB_CUDA(cudaStreamSynchronize(st));
-        edgeCount = 2u * kept;
+        edgeCount = 2u * readBack(totalDev, st);
     }
-    uint32_t* edges = (uint32_t*)(hb.p[2] = allocHostResult(16ull * edgeCount + 16));
-    uint32_t* data = (uint32_t*)(hb.p[3] = allocHostResult(4ull * (2ull * edgeCount) + 4));
-    SHB_REQUIRE(edges && data, SHB_ERR_OOM, "Out of host memory for the read graph.");
+    HostResult edgesBlock(allocHostResult(16ull * edgeCount + 16)), dataBlock(allocHostResult(4ull * (2ull * edgeCount) + 4));
+    SHB_REQUIRE(edgesBlock.p && dataBlock.p, SHB_ERR_OOM, "Out of host memory for the read graph.");
     if(edgeCount == 0) {
         memset(toc, 0, 4ull * (uint64_t(rows) + 1));
         memset(keepHost, 0, n);
@@ -231,15 +212,14 @@ void createReadGraph(shb_context* c, void* alignmentData, uint64_t n, uint64_t r
         // the item buffers are free again: reuse them for the (row, edge) entries
         SHB_LAUNCH(readGraphEdgesKernel, ceilDiv(n, 256), 256, 0, st, (const uint32_t*)dRec.get(), uint32_t(n), (const uint32_t*)keep.get(),
                    (const uint32_t*)keepIndex.get(), entries, dEdges.get(), keysA.get(), valsA.get());
-        uint32_t rowBits = 1;
-        while((1ull << rowBits) < uint64_t(rows)) rowBits++;
+        const uint32_t rowBits = bitsFor(rows ? rows - 1 : 0);
         const int ranges[1][2] = {{32, 32 + int(rowBits)}};
         const bool inB = radixSort<true>(keysA.get(), keysB.get(), valsA.get(), valsB.get(), entries, ranges, 1, c->sortWs, st);
-        SHB_LAUNCH(readGraphTocKernel, ceilDiv(uint64_t(rows) + 1, 256), 256, 0, st, (const uint64_t*)(inB ? keysB.get() : keysA.get()),
+        SHB_LAUNCH(rowStartsKernel<uint32_t>, ceilDiv(uint64_t(rows) + 1, 256), 256, 0, st, (const uint64_t*)(inB ? keysB.get() : keysA.get()),
                    entries, rows, dToc.get());
         SHB_CUDA(cudaMemcpyAsync(toc, dToc.get(), 4ull * (uint64_t(rows) + 1), cudaMemcpyDeviceToHost, st));
-        SHB_CUDA(cudaMemcpyAsync(data, inB ? valsB.get() : valsA.get(), 4ull * entries, cudaMemcpyDeviceToHost, st));
-        SHB_CUDA(cudaMemcpyAsync(edges, dEdges.get(), 16ull * edgeCount, cudaMemcpyDeviceToHost, st));
+        SHB_CUDA(cudaMemcpyAsync(dataBlock.p, inB ? valsB.get() : valsA.get(), 4ull * entries, cudaMemcpyDeviceToHost, st));
+        SHB_CUDA(cudaMemcpyAsync(edgesBlock.p, dEdges.get(), 16ull * edgeCount, cudaMemcpyDeviceToHost, st));
         // keep flags as bytes: narrow on the host (n words)
         std::vector<uint32_t> keepWords(n);
         SHB_CUDA(cudaMemcpyAsync(keepWords.data(), keep.get(), 4ull * n, cudaMemcpyDeviceToHost, st));
@@ -263,8 +243,8 @@ void createReadGraph(shb_context* c, void* alignmentData, uint64_t n, uint64_t r
         uint32_t& w = rec[kAlignmentWords * i + 15];
         w = (w & ~1u) | uint32_t(keepHost[i] & 1u);
     }
-    *keepOut = keepHost; *edgesOut = edges; *edgeCountOut = edgeCount; *connectivityTocOut = toc; *connectivityDataOut = data;
-    hb.disarm();
+    *keepOut = static_cast<uint8_t*>(keepBlock.take()); *edgesOut = edgesBlock.take(); *edgeCountOut = edgeCount;
+    *connectivityTocOut = static_cast<uint32_t*>(tocBlock.take()); *connectivityDataOut = static_cast<uint32_t*>(dataBlock.take());
 }
 
 } // namespace shb

@@ -296,17 +296,6 @@ __global__ void regionRootKernel(uint32_t* parent, uint32_t rows, const uint8_t*
     if(v < rows) root[v] = nearRead[v >> 1] == kYes ? findRoot(parent, v) : kEmpty;
 }
 
-struct Footprint {
-    uint64_t live = 0, peak = 0;
-    template<class T> void add(DeviceBuffer<T>& b, uint64_t n)
-    {
-        const uint64_t before = b.capacity();
-        b.reserve(n);
-        live += (b.capacity() - before) * sizeof(T);
-        peak = std::max(peak, live);
-    }
-};
-
 struct DeviceGraph {
     DeviceBuffer<uint32_t> toc, adj, edges, scratch;
 };
@@ -340,13 +329,11 @@ void buildGraph(shb_context* c, const uint32_t* edges, uint64_t edgeCount, const
     if(entries) {
         uint32_t* dData = g.scratch.get();
         SHB_CUDA(cudaMemcpyAsync(dData, connData, 4ull * entries, cudaMemcpyHostToDevice, st));
-        uint32_t* bad = reinterpret_cast<uint32_t*>(c->scalars.get());
+        uint32_t* bad = reinterpret_cast<uint32_t*>(c->scalar(kSlotBadConnectivity));
         SHB_CUDA(cudaMemsetAsync(bad, 0, 4, st));
         SHB_LAUNCH(adjacencyKernel, ceilDiv(entries, 256), 256, 0, st, (const uint32_t*)g.toc.get(), uint32_t(rows), (const uint32_t*)dData,
                    entries, (const uint32_t*)g.edges.get(), edgeCount, keepCross, g.adj.get(), bad);
-        uint32_t badHost = 0;
-        SHB_CUDA(cudaMemcpyAsync(&badHost, bad, 4, cudaMemcpyDeviceToHost, st));
-        SHB_CUDA(cudaStreamSynchronize(st));
+        const uint32_t badHost = readBack(bad, st);
         SHB_REQUIRE(badHost == 0, SHB_ERR_INVALID, std::to_string(badHost) +
                     " ReadGraphConnectivity entries name an edge that does not exist or does not touch their oriented read.");
     }
@@ -497,11 +484,6 @@ void processRegion(const std::vector<uint32_t>& vertices, const uint32_t* edges,
             }
         }
     }
-}
-
-double msSince(std::chrono::steady_clock::time_point t0)
-{
-    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
 }
 
 } // namespace

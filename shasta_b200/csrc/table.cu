@@ -29,27 +29,6 @@ __global__ void pairTableKeysKernel(const uint32_t* __restrict__ records, uint32
     keys[4ull * i + 3] = (uint64_t(o1 ^ 1u) << 32) | (o0 ^ 1u); vals[4ull * i + 3] = i;
 }
 
-template<class T> __global__ void pairTableTocKernel(const uint64_t* __restrict__ sortedKeys, uint32_t entries, uint32_t rows, T* __restrict__ toc)
-{
-    const uint32_t row = blockIdx.x * blockDim.x + threadIdx.x;
-    if(row > rows) return;
-    uint32_t lo = 0, hi = entries;          // first entry whose row is >= this row
-    while(lo < hi) { const uint32_t mid = lo + ((hi - lo) >> 1); if(uint32_t(sortedKeys[mid] >> 32) < row) lo = mid + 1; else hi = mid; }
-    toc[row] = T(lo);
-}
-
-__global__ void widenKernel(const uint32_t* __restrict__ in, uint32_t n, unsigned long long* __restrict__ out)
-{
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if(i < n) out[i] = in[i];
-}
-
-struct HostBlocks {         // frees what was not handed to the caller (error paths)
-    void* p[2] = {nullptr, nullptr};
-    ~HostBlocks() { for(void* q : p) if(q) HostPool::instance().release(q); }
-    void disarm() { p[0] = p[1] = nullptr; }
-};
-
 // T = uint32_t (alignment table) or unsigned long long (candidate table).
 template<class T> void computePairTable(shb_context* c, const uint32_t* rec, uint32_t stride, uint64_t n, uint64_t readCount,
                                         T** tocOut, T** dataOut, const char* what)
@@ -59,13 +38,11 @@ template<class T> void computePairTable(shb_context* c, const uint32_t* rec, uin
     SHB_CUDA(cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const uint32_t rows = uint32_t(2 * readCount);
-    HostBlocks hb;
-    T* toc = (T*)(hb.p[0] = allocHostResult(sizeof(T) * (uint64_t(rows) + 1)));
-    T* data = (T*)(hb.p[1] = allocHostResult(sizeof(T) * (4 * n + 1)));
-    SHB_REQUIRE(toc && data, SHB_ERR_OOM, "Out of host memory for the table.");
+    HostResult tocHost(allocHostResult(sizeof(T) * (uint64_t(rows) + 1))), dataHost(allocHostResult(sizeof(T) * (4 * n + 1)));
+    SHB_REQUIRE(tocHost.p && dataHost.p, SHB_ERR_OOM, "Out of host memory for the table.");
     if(n == 0) {
-        memset(toc, 0, sizeof(T) * (uint64_t(rows) + 1));
-        *tocOut = toc; *dataOut = data; hb.disarm();
+        memset(tocHost.p, 0, sizeof(T) * (uint64_t(rows) + 1));
+        *tocOut = static_cast<T*>(tocHost.take()); *dataOut = static_cast<T*>(dataHost.take());
         return;
     }
     for(uint64_t i = 0; i < n; i++) {
@@ -80,23 +57,22 @@ template<class T> void computePairTable(shb_context* c, const uint32_t* rec, uin
     dToc.reserve(uint64_t(rows) + 1);
     SHB_CUDA(cudaMemcpyAsync(dRec.get(), rec, 4ull * stride * n, cudaMemcpyHostToDevice, st));
     SHB_LAUNCH(pairTableKeysKernel, ceilDiv(n, 256), 256, 0, st, (const uint32_t*)dRec.get(), stride, uint32_t(n), keysA.get(), valsA.get());
-    uint32_t rowBits = 1;
-    while((1ull << rowBits) < uint64_t(rows)) rowBits++;
+    const uint32_t rowBits = bitsFor(rows ? rows - 1 : 0);
     const int ranges[2][2] = {{0, int(rowBits)}, {32, 32 + int(rowBits)}};
     const bool inB = radixSort<true>(keysA.get(), keysB.get(), valsA.get(), valsB.get(), entries, ranges, 2, c->sortWs, st);
-    SHB_LAUNCH((pairTableTocKernel<T>), ceilDiv(uint64_t(rows) + 1, 256), 256, 0, st, (const uint64_t*)(inB ? keysB.get() : keysA.get()),
+    SHB_LAUNCH((rowStartsKernel<T>), ceilDiv(uint64_t(rows) + 1, 256), 256, 0, st, (const uint64_t*)(inB ? keysB.get() : keysA.get()),
                entries, rows, dToc.get());
-    SHB_CUDA(cudaMemcpyAsync(toc, dToc.get(), sizeof(T) * (uint64_t(rows) + 1), cudaMemcpyDeviceToHost, st));
+    SHB_CUDA(cudaMemcpyAsync(tocHost.p, dToc.get(), sizeof(T) * (uint64_t(rows) + 1), cudaMemcpyDeviceToHost, st));
     const uint32_t* sortedVals = inB ? valsB.get() : valsA.get();
     if(sizeof(T) == 4) {
-        SHB_CUDA(cudaMemcpyAsync(data, sortedVals, 4ull * entries, cudaMemcpyDeviceToHost, st));
+        SHB_CUDA(cudaMemcpyAsync(dataHost.p, sortedVals, 4ull * entries, cudaMemcpyDeviceToHost, st));
     } else {
         dWide.reserve(entries);
-        SHB_LAUNCH(widenKernel, ceilDiv(entries, 256), 256, 0, st, sortedVals, entries, (unsigned long long*)dWide.get());
-        SHB_CUDA(cudaMemcpyAsync(data, dWide.get(), 8ull * entries, cudaMemcpyDeviceToHost, st));
+        SHB_LAUNCH(widenKernel<uint32_t>, ceilDiv(entries, 256), 256, 0, st, sortedVals, entries, (unsigned long long*)dWide.get());
+        SHB_CUDA(cudaMemcpyAsync(dataHost.p, dWide.get(), 8ull * entries, cudaMemcpyDeviceToHost, st));
     }
     SHB_CUDA(cudaStreamSynchronize(st));
-    *tocOut = toc; *dataOut = data; hb.disarm();
+    *tocOut = static_cast<T*>(tocHost.take()); *dataOut = static_cast<T*>(dataHost.take());
 }
 
 } // namespace

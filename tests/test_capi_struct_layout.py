@@ -1,4 +1,5 @@
-"""The ctypes mirrors in shasta_b200/capi.py against include/shasta_b200.h: sizes and field offsets as gcc lays the C structs out."""
+"""The ctypes mirrors in shasta_b200/capi.py against include/shasta_b200.h: sizes and field offsets as gcc lays the C structs out,
+for every struct the header defines."""
 import ctypes as C
 import os
 import re
@@ -9,7 +10,17 @@ from shasta_b200 import capi
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PAIRS = {"shb_lowhash_params": capi.LowHashParams, "shb_lowhash_result": capi.LowHashResult, "shb_align_options": capi.AlignOptions,
          "shb_align_result": capi.AlignResult, "shb_marker_result": capi.MarkerResult, "shb_dist_timing": capi.DistTiming,
-         "shb_read_graph2_criteria": capi.ReadGraph2Criteria}
+         "shb_read_graph2_criteria": capi.ReadGraph2Criteria, "shb_cross_strand_result": capi.CrossStrandResult,
+         "shb_chimeric_result": capi.ChimericResult, "shb_palindromic_params": capi.PalindromicParams,
+         "shb_palindromic_result": capi.PalindromicResult, "shb_marker_graph_params": capi.MarkerGraphParams,
+         "shb_marker_graph_result": capi.MarkerGraphResult}
+
+
+def test_every_header_struct_has_a_mirror():
+    text = re.sub(r"/\*.*?\*/", "", open(os.path.join(ROOT, "include", "shasta_b200.h")).read(), flags=re.S)
+    defined = set(re.findall(r"typedef\s+struct\s*\w*\s*\{[^}]*\}\s*(shb_\w+)\s*;", text))
+    assert "shb_context" not in defined      # opaque: declared, never defined
+    assert len(defined) == 13 and defined == set(PAIRS)
 
 
 def test_struct_sizes_and_offsets(tmp_path):

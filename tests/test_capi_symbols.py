@@ -58,15 +58,15 @@ def declared_parameter_counts():
 
 
 def test_ctypes_argument_lists_match_the_header():
-    """Every binding that declares argtypes passes as many arguments as the prototype in include/shasta_b200.h has."""
+    """capi.lib() declares the argtypes of every function in include/shasta_b200.h that has parameters when it loads the
+    library, and each passes as many arguments as the prototype has."""
     from shasta_b200 import capi
     lib = capi.lib()
     counts = declared_parameter_counts()
     assert counts["shb_lowhash0"] == 8 and counts["shb_last_error"] == 0
-    checked = 0
     for name, n in counts.items():
         argtypes = getattr(lib, name).argtypes
+        if n:
+            assert argtypes is not None, f"{name}: no ctypes argument list"
         if argtypes is not None:
             assert len(argtypes) == n, f"{name}: {len(argtypes)} ctypes arguments, {n} in the header"
-            checked += 1
-    assert checked >= 15

@@ -1,8 +1,6 @@
 """GPU test of the library's own radix sort (csrc/radix_sort.cuh: one kernel per 8-bit pass, decoupled look-back) against
 numpy's stable sort, through the test hook shb_test_radix_sort: sizes around the 4096-item tile, many tiles (look-back
 chains), skewed digits, one and two bit ranges, with and without a payload, repeated calls (status tags)."""
-import ctypes as C
-
 import numpy as np
 import pytest
 
@@ -13,7 +11,6 @@ pytestmark = pytest.mark.gpu
 def ctx():
     from shasta_b200 import capi
     c = capi.Context(0)
-    capi.lib().shb_test_radix_sort.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_int]
     yield c
     c.close()
 

@@ -3,11 +3,8 @@ against the reference's own DisjointSets, decompress and PeakFinder driven in th
 (oracle/ref_glue/ref_markergraph.cpp), in canonical form (vertices by first marker). PeakFinder alone: the library's
 restatement (shb_peak_finder_cutoff) and the oracle's against the reference on a few hundred histograms. The reference's
 outputs are stored in tests/golden/reference_markergraph.npz."""
-import ctypes as C
 import hashlib
 import os
-import re
-import subprocess
 import sys
 
 import numpy as np
@@ -19,7 +16,6 @@ sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "gol
 from markergraph_inputs import PARAMS, START_INDEX, cases, histograms  # noqa: E402
 from reference_outputs import recorded  # noqa: E402
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CASES = cases()
 HISTOGRAMS = histograms()
 
@@ -145,26 +141,3 @@ def MB_first_ordinal(d):
     from oracle import bindings as B
     a = int(d["edges"][0, 2])
     return B.oracle_decompress(d["cdata"][int(d["ctoc"][a]):int(d["ctoc"][a + 1])])[0, 0]
-
-
-def test_struct_layout(tmp_path):
-    """The new structs against their ctypes mirrors, as gcc lays them out."""
-    from shasta_b200 import capi
-    pairs = {"shb_marker_graph_params": capi.MarkerGraphParams, "shb_marker_graph_result": capi.MarkerGraphResult}
-    lines = ['#include <stdio.h>', '#include <stddef.h>', '#include "shasta_b200.h"', 'int main(void) {']
-    for cname, cls in pairs.items():
-        lines.append(f'printf("{cname} size %zu\\n", sizeof({cname}));')
-        for field, _ in cls._fields_:
-            lines.append(f'printf("{cname} {field} %zu\\n", offsetof({cname}, {field}));')
-    lines.append("return 0; }")
-    src = tmp_path / "layout.c"
-    src.write_text("\n".join(lines))
-    exe = tmp_path / "layout"
-    subprocess.check_call(["gcc", "-std=c11", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)])
-    seen = 0
-    for line in subprocess.check_output([str(exe)], text=True).splitlines():
-        cname, what, value = re.match(r"(\w+) (\w+) (\d+)", line).groups()
-        cls = pairs[cname]
-        assert (C.sizeof(cls) if what == "size" else getattr(cls, what).offset) == int(value), (cname, what)
-        seen += 1
-    assert seen == sum(len(c._fields_) + 1 for c in pairs.values())
