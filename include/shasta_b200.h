@@ -530,4 +530,7 @@ shb_status shb_copy_device_to_host(void* dstHost, const void* srcDevice, uint64_
 #ifdef __cplusplus
 }
 #endif
+
+/* createMarkerGraphEdges and findMarkerGraphReverseComplementEdges: shb_marker_graph_edges_result and their entry points. */
+#include "shb_marker_graph_edges.h"
 #endif

@@ -27,6 +27,7 @@ import numpy as np
 
 MAGIC = 0xa3756fd4b5d8bcc1
 HEADER_BYTES = 4096
+EDGE_BYTES = 14                 # sizeof(MarkerGraph::Edge) (src/MarkerGraph.hpp:179-244)
 
 
 def mm_write_vector(path, array, object_size=None, page_size=4096):
@@ -534,6 +535,69 @@ class Assembler:
         except capi.ShastaB200Error as e:
             raise RuntimeError(str(e)) from None
         mm_write_vector(self._name("MarkerGraphReverseComplementeVertex"), rc, object_size=8, page_size=self.page_size)
+
+    # ------------------------------------------------------------------ marker graph edges
+    def createMarkerGraphEdges(self, threadCount=0):
+        """Assembler::createMarkerGraphEdges (src/AssemblerMarkerGraph.cpp:2028-2213) on Data/MarkerGraphVertexTable and
+        Data/MarkerGraphVertices.{toc,data}. Writes Data/GlobalMarkerGraphEdges (14-byte Edge records),
+        Data/GlobalMarkerGraphEdgeMarkerIntervals.{toc,data} (VectorOfVectors<MarkerInterval, uint64_t>) and
+        Data/GlobalMarkerGraphEdgesBySource / ...ByTarget.{toc,data} (VectorOfVectors<Uint40, uint64_t>), as the reference
+        run with one thread writes them, and prints the reference's line. threadCount is ignored."""
+        from . import capi
+        self.checkMarkersAreOpen()
+        self.accessMarkerGraphVertices()
+        table, vtoc, vdata = self._marker_graph
+        ctx = self._upload_markers()
+        try:
+            out, res = capi.create_marker_graph_edges(ctx, table, vtoc, vdata)
+        except capi.ShastaB200Error as e:
+            raise RuntimeError(str(e)) from None
+        print(f"Found {res.edgeCount} edges for {res.vertexCount} vertices.")
+        self._write_marker_graph_edges(out)
+        self._marker_graph_edges = out
+
+    def _write_marker_graph_edges(self, out):
+        ps = self.page_size
+        mm_write_vector(self._name("GlobalMarkerGraphEdges"), out["edges"], object_size=EDGE_BYTES, page_size=ps)
+        mm_write_vector_of_vectors(self._name("GlobalMarkerGraphEdgeMarkerIntervals"), out["intervalsToc"], out["intervalsData"],
+                                   data_object_size=12, page_size=ps)
+        for name, key in (("GlobalMarkerGraphEdgesBySource", "bySource"), ("GlobalMarkerGraphEdgesByTarget", "byTarget")):
+            mm_write_vector_of_vectors(self._name(name), out[key + "Toc"], out[key + "Data"], data_object_size=5, page_size=ps)
+
+    def accessMarkerGraphEdges(self, accessEdgesReadWrite=False, accessConnectivityReadWrite=False):
+        """The five edge file sets createMarkerGraphEdges writes (read only here: the flags say how the reference maps them)."""
+        itoc = mm_read_vector(self._name("GlobalMarkerGraphEdgeMarkerIntervals.toc"), np.uint64, object_size=8)
+        self._marker_graph_edges = dict(
+            edges=np.asarray(mm_read_vector(self._name("GlobalMarkerGraphEdges"), np.uint8, object_size=EDGE_BYTES)).reshape(-1, 14),
+            intervalsToc=np.asarray(itoc),
+            intervalsData=np.asarray(mm_read_vector(self._name("GlobalMarkerGraphEdgeMarkerIntervals.data"), np.uint32,
+                                                    object_size=12)).reshape(-1, 3),
+            bySourceToc=np.asarray(mm_read_vector(self._name("GlobalMarkerGraphEdgesBySource.toc"), np.uint64, object_size=8)),
+            bySourceData=np.asarray(mm_read_vector(self._name("GlobalMarkerGraphEdgesBySource.data"), np.uint8, object_size=5)),
+            byTargetToc=np.asarray(mm_read_vector(self._name("GlobalMarkerGraphEdgesByTarget.toc"), np.uint64, object_size=8)),
+            byTargetData=np.asarray(mm_read_vector(self._name("GlobalMarkerGraphEdgesByTarget.data"), np.uint8, object_size=5)))
+
+    def findMarkerGraphReverseComplementEdges(self, threadCount=0):
+        """Assembler::findMarkerGraphReverseComplementEdges (:1244-1389) on the edges of this session or of accessMarkerGraphEdges
+        and on Data/MarkerGraphReverseComplementeVertex. Writes Data/MarkerGraphReverseComplementeEdge (the reference's file
+        name), uint64 per edge. Works on edges in any numbering, parallel edges included. threadCount is ignored."""
+        from . import capi
+        edges = getattr(self, "_marker_graph_edges", None)
+        if edges is None:
+            raise RuntimeError("Marker graph edges are not accessible.")
+        rc_vertex = mm_read_vector(self._name("MarkerGraphReverseComplementeVertex"), np.uint64, object_size=8)
+        ctx = self._upload_markers()
+        try:
+            rc, _ = capi.find_marker_graph_reverse_complement_edges(ctx, rc_vertex, edges["edges"], edges["intervalsToc"],
+                                                                    edges["intervalsData"], edges["bySourceToc"], edges["bySourceData"])
+        except capi.ShastaB200Error as e:
+            raise RuntimeError(str(e)) from None
+        mm_write_vector(self._name("MarkerGraphReverseComplementeEdge"), rc, object_size=8, page_size=self.page_size)
+        self._marker_graph_rc_edge = rc
+
+    def accessMarkerGraphReverseComplementEdge(self):
+        """Data/MarkerGraphReverseComplementeEdge: uint64 per edge."""
+        self._marker_graph_rc_edge = np.asarray(mm_read_vector(self._name("MarkerGraphReverseComplementeEdge"), np.uint64, object_size=8))
 
 
 def write_disjoint_sets_histogram_csv(path, histogram):

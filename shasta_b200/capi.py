@@ -171,6 +171,11 @@ def lib():
                                                        C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(MarkerGraphResult)]
         L.shb_find_marker_graph_reverse_complement_vertices.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
                                                                         C.POINTER(C.c_void_p)]
+        L.shb_create_marker_graph_edges.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64] + \
+            [C.POINTER(C.c_void_p)] * 7 + [C.POINTER(MarkerGraphEdgesResult)]
+        L.shb_find_marker_graph_reverse_complement_edges.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p,
+                                                                     C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p),
+                                                                     C.POINTER(MarkerGraphEdgesResult)]
         L.shb_peak_finder_cutoff.restype = C.c_int
         L.shb_peak_finder_cutoff.argtypes = [C.c_void_p, C.c_uint64, C.c_double, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_double)]
         _lib = L
@@ -682,3 +687,52 @@ def peak_finder_cutoff(histogram, min_area_fraction=0.08, start_index=2):
     cutoff, observed = C.c_uint64(0), C.c_double(0)
     threw = lib().shb_peak_finder_cutoff(_ptr(y) if len(y) else None, len(y), float(min_area_fraction), int(start_index), C.byref(cutoff), C.byref(observed))
     return int(threw), int(cutoff.value), float(observed.value)
+
+
+# ---- createMarkerGraphEdges, findMarkerGraphReverseComplementEdges (include/shb_marker_graph_edges.h) -------------------
+class MarkerGraphEdgesResult(_Struct):
+    _fields_ = [("vertexCount", C.c_uint64), ("edgeCount", C.c_uint64), ("markerIntervalCount", C.c_uint64),
+                ("saturatedEdgeCount", C.c_uint64), ("peakDeviceBytes", C.c_uint64), ("kernelLaunches", C.c_uint64),
+                ("deviceMs", C.c_double), ("totalMs", C.c_double)]
+
+
+EDGE_BYTES = 14         # sizeof(MarkerGraph::Edge): Uint40 source, Uint40 target, coverage, flag bytes
+
+
+def create_marker_graph_edges(ctx: Context, vertex_table, vertices_toc, vertices_data):
+    """Assembler::createMarkerGraphEdges with createMarkerGraphEdgesBySourceAndTarget on the markers ctx holds.
+    vertex_table / vertices_toc: Uint40 bytes; vertices_data: uint64. Returns dict(edges uint8[E,14], intervalsToc uint64[E+1],
+    intervalsData uint32[I,3], bySourceToc uint64[V+1], bySourceData uint8[5E] (Uint40), byTargetToc, byTargetData) and the
+    MarkerGraphEdgesResult."""
+    t = np.ascontiguousarray(vertex_table, np.uint8)
+    vt = np.ascontiguousarray(vertices_toc, np.uint8)
+    vd = np.ascontiguousarray(vertices_data, np.uint64)
+    V = len(vt) // 5 - 1
+    ptrs = [C.c_void_p() for _ in range(7)]
+    res = MarkerGraphEdgesResult()
+    _check(lib().shb_create_marker_graph_edges(ctx._h, _ptr(t), len(t) // 5, _ptr(vt), _ptr(vd), V, *[C.byref(p) for p in ptrs],
+                                               C.byref(res)))
+    E, I = res.edgeCount, res.markerIntervalCount
+    out = dict(edges=_owned_array(ptrs[0], EDGE_BYTES * E, np.uint8).reshape(-1, EDGE_BYTES),
+               intervalsToc=_owned_array(ptrs[1], E + 1, np.uint64), intervalsData=_owned_array(ptrs[2], 3 * I, np.uint32).reshape(-1, 3),
+               bySourceToc=_owned_array(ptrs[3], V + 1, np.uint64), bySourceData=_owned_array(ptrs[4], 5 * E, np.uint8),
+               byTargetToc=_owned_array(ptrs[5], V + 1, np.uint64), byTargetData=_owned_array(ptrs[6], 5 * E, np.uint8))
+    return out, res
+
+
+def find_marker_graph_reverse_complement_edges(ctx: Context, rc_vertex, edges, intervals_toc, intervals_data, by_source_toc,
+                                               by_source_data):
+    """Assembler::findMarkerGraphReverseComplementEdges. edges: uint8[E,14] records; intervals_data: uint32[I,3];
+    by_source_data: Uint40 bytes. Returns (uint64[E], MarkerGraphEdgesResult)."""
+    rv = np.ascontiguousarray(rc_vertex, np.uint64)
+    e = np.ascontiguousarray(edges, np.uint8).reshape(-1)
+    it = np.ascontiguousarray(intervals_toc, np.uint64)
+    iv = np.ascontiguousarray(intervals_data, np.uint32).reshape(-1)
+    st = np.ascontiguousarray(by_source_toc, np.uint64)
+    sd = np.ascontiguousarray(by_source_data, np.uint8)
+    E = len(e) // EDGE_BYTES
+    rc = C.c_void_p()
+    res = MarkerGraphEdgesResult()
+    _check(lib().shb_find_marker_graph_reverse_complement_edges(ctx._h, _ptr(rv), len(rv), _ptr(e), E, _ptr(it), _ptr(iv), _ptr(st),
+                                                                _ptr(sd), C.byref(rc), C.byref(res)))
+    return _owned_array(rc, E, np.uint64), res

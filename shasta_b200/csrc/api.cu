@@ -51,6 +51,12 @@ void createMarkerGraphVertices(shb_context* c, const shb_marker_graph_params& p,
                                shb_marker_graph_result* result);
 void findMarkerGraphReverseComplementVertices(shb_context* c, const uint8_t* table5, const uint8_t* toc5, const uint64_t* vdata,
                                               uint64_t V, uint64_t** rcOut);
+void createMarkerGraphEdges(shb_context* c, const uint8_t* table5, uint64_t tableCount, const uint8_t* toc5, const uint64_t* vdata,
+                            uint64_t V, uint8_t** edgesOut, uint64_t** itocOut, uint8_t** idataOut, uint64_t** stocOut,
+                            uint8_t** sdataOut, uint64_t** ttocOut, uint8_t** tdataOut, shb_marker_graph_edges_result* result);
+void findMarkerGraphReverseComplementEdges(shb_context* c, const uint64_t* rcVertex, uint64_t V, const uint8_t* edges, uint64_t E,
+                                           const uint64_t* itoc, const uint8_t* idata, const uint64_t* stoc, const uint8_t* sdata,
+                                           uint64_t** rcOut, shb_marker_graph_edges_result* result);
 void flagCrossStrandReadGraphEdges1(shb_context* c, int64_t maxDistance, uint32_t* edges, uint64_t edgeCount, const uint32_t* connToc,
                                     const uint32_t* connData, uint64_t readCount, uint32_t* rec, uint64_t alignmentCount,
                                     shb_cross_strand_result* result);
@@ -510,6 +516,37 @@ shb_status shb_find_marker_graph_reverse_complement_vertices(shb_context* c, con
     return guarded([&] {
         SHB_REQUIRE(c && verticesToc && rcVertex && ((vertexTable && verticesData) || vertexCount == 0), SHB_ERR_INVALID, "Null argument.");
         findMarkerGraphReverseComplementVertices(c, vertexTable, verticesToc, verticesData, vertexCount, rcVertex);
+    });
+}
+
+shb_status shb_create_marker_graph_edges(shb_context* c, const uint8_t* vertexTable, uint64_t vertexTableCount,
+                                         const uint8_t* verticesToc, const uint64_t* verticesData, uint64_t vertexCount,
+                                         uint8_t** edges, uint64_t** intervalsToc, uint8_t** intervalsData,
+                                         uint64_t** bySourceToc, uint8_t** bySourceData, uint64_t** byTargetToc,
+                                         uint8_t** byTargetData, shb_marker_graph_edges_result* result)
+{
+    return guarded([&] {
+        SHB_REQUIRE(c && (vertexTable || vertexTableCount == 0) && verticesToc && (verticesData || vertexCount == 0) && edges &&
+                    intervalsToc && intervalsData && bySourceToc && bySourceData && byTargetToc && byTargetData, SHB_ERR_INVALID,
+                    "Null argument.");
+        createMarkerGraphEdges(c, vertexTable, vertexTableCount, verticesToc, verticesData, vertexCount, edges, intervalsToc,
+                               intervalsData, bySourceToc, bySourceData, byTargetToc, byTargetData, result);
+    });
+}
+
+shb_status shb_find_marker_graph_reverse_complement_edges(shb_context* c, const uint64_t* rcVertex, uint64_t vertexCount,
+                                                          const uint8_t* edges, uint64_t edgeCount, const uint64_t* intervalsToc,
+                                                          const uint8_t* intervalsData, const uint64_t* bySourceToc,
+                                                          const uint8_t* bySourceData, uint64_t** rcEdge,
+                                                          shb_marker_graph_edges_result* result)
+{
+    return guarded([&] {
+        SHB_REQUIRE(c && (rcVertex || vertexCount == 0) && (edges || edgeCount == 0) && intervalsToc && bySourceToc && rcEdge,
+                    SHB_ERR_INVALID, "Null argument.");
+        SHB_REQUIRE(intervalsData || intervalsToc[edgeCount] == 0, SHB_ERR_INVALID, "Null argument.");
+        SHB_REQUIRE(bySourceData || bySourceToc[vertexCount] == 0, SHB_ERR_INVALID, "Null argument.");
+        findMarkerGraphReverseComplementEdges(c, rcVertex, vertexCount, edges, edgeCount, intervalsToc, intervalsData, bySourceToc,
+                                              bySourceData, rcEdge, result);
     });
 }
 

@@ -35,7 +35,10 @@ enum ScalarSlot : uint32_t {
     kSlotBadConnectivity,                                       // readgraph_flags: bad ReadGraphConnectivity entries (uint32)
     kSlotMarkerGraphVertices,                                   // markergraph: errKmer, errFormat, alignedCount, maxSize, scan total, bigCount
     kSlotMarkerGraphRcErrors = kSlotMarkerGraphVertices + 6,    // markergraph: errMarker, errVertex
-    kScalarSlotEnd = kSlotMarkerGraphRcErrors + 2
+    kSlotMarkerGraphEdges = kSlotMarkerGraphRcErrors + 2,      // markergraph_edges: errMarker, errOrder, errVertex, longCount,
+                                                                //   bigCount, saturated, edge total, interval total
+    kSlotMarkerGraphRcEdges = kSlotMarkerGraphEdges + 8,        // markergraph_edges: errInput, errAssert, errNotFound, errRcRc
+    kScalarSlotEnd = kSlotMarkerGraphRcEdges + 4
 };
 constexpr uint32_t kScalarWords = 512;                          // reserved once at context creation, never reallocated
 static_assert(kScalarSlotEnd <= kScalarWords, "the scalar slots do not fit the reserved words");
