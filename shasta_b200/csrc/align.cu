@@ -3,7 +3,7 @@
 // Method 4: Align4 front end (cells/components) -> one banded DP per component -> best -> epilogue.
 #include "context.cuh"
 #include "align_kernels.cuh"
-#include "hostpool.cuh"
+#include "hostcopy.cuh"
 #include "digest.cuh"
 
 #include <algorithm>
@@ -175,8 +175,8 @@ struct AlignCache {
     DeviceBuffer<uint32_t> outRecords;
     DeviceBuffer<unsigned long long> outToc;
     DeviceBuffer<uint8_t> outData;
-    cudaStream_t finalStream = nullptr;         // rebase / digest / early device->host copy of the finished batches
-    double lastBytesPerCandidate = 0.;          // compressed bytes per candidate of the previous call (sizes the early copy)
+    cudaStream_t finalStream = nullptr;         // rebase / digest / device->host copy of the finished batches
+    double lastBytesPerCandidate = 0.;          // compressed bytes per candidate of the previous call (sizes the data block)
     ~AlignCache() { if(finalStream) cudaStreamDestroy(finalStream); }
 };
 
@@ -313,52 +313,6 @@ void buildSortedMarkers(shb_context* c, uint32_t k)
     sc.sortedGeneration = c->markerGeneration;
 }
 
-void parallelMemcpy(uint8_t* dst, const uint8_t* src, uint64_t n)
-{
-    constexpr int kThreads = 4;
-    if(n < (4ull << 20)) { memcpy(dst, src, n); return; }
-    std::thread workers[kThreads - 1];
-    const uint64_t part = (n / kThreads + 4095) & ~4095ull;
-    for(int t = 1; t < kThreads; t++) {
-        const uint64_t off = std::min<uint64_t>(n, part * t), len = std::min<uint64_t>(part, n - off);
-        workers[t - 1] = std::thread([=] { if(len) memcpy(dst + off, src + off, len); });
-    }
-    memcpy(dst, src, std::min<uint64_t>(part, n));
-    for(int t = 1; t < kThreads; t++) workers[t - 1].join();
-}
-
-// Device -> pageable host copy through two pinned staging buffers: the DMA of chunk k overlaps the host memcpy of
-// chunk k-1 (a plain cudaMemcpy into pageable memory serialises the two).
-void copyToHostPipelined(shb_context* c, void* dstHost, const void* srcDevice, uint64_t bytes, bool pageLocked)
-{
-    if(bytes == 0) return;
-    if(pageLocked) {        // recycled, page-locked result block: direct DMA
-        SHB_CUDA(cudaMemcpyAsync(dstHost, srcDevice, bytes, cudaMemcpyDeviceToHost, c->stream));
-        return;
-    }
-    constexpr uint64_t kChunk = 32ull << 20;
-    if(!c->pinnedStage[0]) {
-        SHB_CUDA(cudaHostAlloc(&c->pinnedStage[0], kChunk, cudaHostAllocDefault));
-        SHB_CUDA(cudaHostAlloc(&c->pinnedStage[1], kChunk, cudaHostAllocDefault));
-        SHB_CUDA(cudaEventCreateWithFlags(&c->stageEvent[0], cudaEventDisableTiming));
-        SHB_CUDA(cudaEventCreateWithFlags(&c->stageEvent[1], cudaEventDisableTiming));
-    }
-    cudaStream_t st = c->stream;
-    const uint64_t chunks = (bytes + kChunk - 1) / kChunk;
-    for(uint64_t k = 0; k <= chunks; k++) {
-        if(k < chunks) {
-            const uint64_t off = k * kChunk, n = std::min(kChunk, bytes - off);
-            SHB_CUDA(cudaMemcpyAsync(c->pinnedStage[k & 1], static_cast<const uint8_t*>(srcDevice) + off, n, cudaMemcpyDeviceToHost, st));
-            SHB_CUDA(cudaEventRecord(c->stageEvent[k & 1], st));
-        }
-        if(k > 0) {
-            const uint64_t j = k - 1, off = j * kChunk, n = std::min(kChunk, bytes - off);
-            SHB_CUDA(cudaEventSynchronize(c->stageEvent[j & 1]));
-            parallelMemcpy(static_cast<uint8_t*>(dstHost) + off, static_cast<const uint8_t*>(c->pinnedStage[j & 1]), n);
-        }
-    }
-}
-
 // Groups the runnable jobs by band class (longest first inside a class). Returns per-class counts; b.order holds the
 // job indices, class after class.
 void buildClassOrder(AlignWorker& w, const DpJob* jobs, uint32_t nJobs, std::vector<uint64_t>& classCounts, bool forward = false)
@@ -466,14 +420,17 @@ struct AlignCall {
     std::mutex arenaMutex;
     std::map<uint64_t, Segment> ledger;     // by batch index (guarded by arenaMutex)
     uint64_t outCount = 0, outBytes = 0;
-    // Finalisation in candidate order, as soon as a prefix of the batches is complete: rebase, digests and (when the host
-    // result blocks are page-locked and large enough) the device->host copy run on their own stream beside the next batches.
+    // Finalisation in candidate order, as soon as a prefix of the batches is complete: rebase, digests and the device->host
+    // copy run on their own stream beside the next batches.
     cudaStream_t finalStream = nullptr;
     unsigned long long* digests = nullptr;      // device, 2 words
     uint64_t nextToFinalise = 0, finalRecords = 0, finalBytes = 0;
-    uint8_t* hostRecords = nullptr; uint8_t* hostToc = nullptr; uint8_t* hostData = nullptr;     // null: copy at the end
-    uint64_t hostDataCapacity = 0;
-    bool dataOverflow = false;                  // the estimate for the compressed bytes was too small: copy them at the end
+    HostBlock* hostRecords = nullptr; HostBlock* hostToc = nullptr; HostBlock* hostData = nullptr;
+    StagedCopier* copier = nullptr;
+    // the compressed bytes go by direct DMA while they fit the page-locked data block; once they outgrow it, the copier
+    // grows the block and fills the rest
+    bool dataDirect = false;
+    uint64_t dataDirectCapacity = 0;
     // failure of any worker stops the others
     std::atomic<bool> failed{false};
     std::exception_ptr error;
@@ -532,13 +489,22 @@ void finaliseReadySegments(AlignCall& call)
             SHB_LAUNCH(digestCompressedKernel, ceilDiv(seg.kept, 256), 256, 0, fs, (const uint32_t*)ac.outRecords.get() + 16 * seg.recordBase,
                        seg.kept, (const unsigned long long*)segToc, call.finalBytes + seg.bytes,
                        (const uint8_t*)ac.outData.get() + seg.byteBase - call.finalBytes, call.digests + 1);
-            if(call.hostRecords) {
-                SHB_CUDA(cudaMemcpyAsync(call.hostRecords + 64 * call.finalRecords, ac.outRecords.get() + 16 * seg.recordBase, 64 * seg.kept, cudaMemcpyDeviceToHost, fs));
-                SHB_CUDA(cudaMemcpyAsync(call.hostToc + 8 * call.finalRecords, segToc, 8 * seg.kept, cudaMemcpyDeviceToHost, fs));
-                if(!call.dataOverflow && call.finalBytes + seg.bytes <= call.hostDataCapacity) {
-                    SHB_CUDA(cudaMemcpyAsync(call.hostData + call.finalBytes, ac.outData.get() + seg.byteBase, seg.bytes, cudaMemcpyDeviceToHost, fs));
-                } else call.dataOverflow = true;
-            }
+            // The arena may move before a staged copy's DMA is queued: the copier looks the source up under arenaMutex.
+            const AlignCache* acp = &ac;
+            const uint64_t recordBase = seg.recordBase, byteBase = seg.byteBase;
+            if(call.hostRecords->pageLocked) {
+                SHB_CUDA(cudaMemcpyAsync(call.hostRecords->data() + 64 * call.finalRecords, ac.outRecords.get() + 16 * seg.recordBase, 64 * seg.kept, cudaMemcpyDeviceToHost, fs));
+            } else call.copier->copy(*call.hostRecords, 64 * call.finalRecords,
+                                     [acp, recordBase] { return reinterpret_cast<const uint8_t*>(acp->outRecords.get() + 16 * recordBase); }, 64 * seg.kept);
+            if(call.hostToc->pageLocked) {
+                SHB_CUDA(cudaMemcpyAsync(call.hostToc->data() + 8 * call.finalRecords, segToc, 8 * seg.kept, cudaMemcpyDeviceToHost, fs));
+            } else call.copier->copy(*call.hostToc, 8 * call.finalRecords,
+                                     [acp, recordBase] { return reinterpret_cast<const uint8_t*>(acp->outToc.get() + recordBase); }, 8 * seg.kept);
+            if(call.dataDirect && call.finalBytes + seg.bytes > call.dataDirectCapacity) call.dataDirect = false;
+            if(call.dataDirect) {
+                SHB_CUDA(cudaMemcpyAsync(call.hostData->data() + call.finalBytes, ac.outData.get() + seg.byteBase, seg.bytes, cudaMemcpyDeviceToHost, fs));
+            } else call.copier->copy(*call.hostData, call.finalBytes,
+                                     [acp, byteBase] { return acp->outData.get() + byteBase; }, seg.bytes);
             call.finalRecords += seg.kept; call.finalBytes += seg.bytes;
         }
         call.nextToFinalise++;
@@ -860,19 +826,15 @@ void computeAlignments(shb_context* c, const void* candidatesHost, uint64_t n, c
     call.finalStream = ac.finalStream;
     call.digests = c->scalar(kSlotAlignmentDigests);
     SHB_CUDA(cudaMemsetAsync(call.digests, 0, 2 * sizeof(unsigned long long), st));
-    // Host result blocks up front when recycled, page-locked blocks are available (every call after the first of a steady
-    // caller): records and toc by their upper bound (every candidate kept), the compressed bytes by the previous call's bytes per
-    // candidate. The finished prefix of the batches is then copied out while the later batches run.
-    HostResult recOut, tocOut, dataOut;
-    if(n && ac.lastBytesPerCandidate > 0.) {
-        const uint64_t dataEstimate = uint64_t(ac.lastBytesPerCandidate * double(n) * 1.03) + (1ull << 20);
-        recOut.reset(allocHostResult(64 * n)); tocOut.reset(allocHostResult(8 * (n + 1))); dataOut.reset(allocHostResult(dataEstimate));
-        if(recOut.p && tocOut.p && dataOut.p && HostPool::instance().isPageLocked(recOut.p) && HostPool::instance().isPageLocked(tocOut.p) &&
-           HostPool::instance().isPageLocked(dataOut.p)) {
-            call.hostRecords = static_cast<uint8_t*>(recOut.p); call.hostToc = static_cast<uint8_t*>(tocOut.p);
-            call.hostData = static_cast<uint8_t*>(dataOut.p); call.hostDataCapacity = dataEstimate;
-        }
-    }
+    // Host result blocks up front: records and toc by their upper bound (every candidate kept), the compressed bytes by the
+    // previous call's bytes per candidate (a guess on the first call; the copier grows the block when it falls short). Only
+    // the pages written are touched. The finished prefix of the batches is copied out while the later batches run: by direct
+    // DMA into page-locked blocks (recycled ones), through the staging ring and four copier threads into the others.
+    const uint64_t dataEstimate = n ? uint64_t((ac.lastBytesPerCandidate > 0. ? ac.lastBytesPerCandidate * 1.03 : 64.) * double(n)) + (1ull << 20) : 0;
+    HostBlock recOut(64 * n), tocOut(8 * (n + 1)), dataOut(dataEstimate);
+    StagedCopier copier(c, call.finalStream, 4, &call.arenaMutex);
+    call.hostRecords = &recOut; call.hostToc = &tocOut; call.hostData = &dataOut; call.copier = &copier;
+    call.dataDirect = dataOut.pageLocked; call.dataDirectCapacity = dataEstimate;
     SHB_CUDA(cudaStreamSynchronize(st));        // derived marker data ready before the workers read it
 
     if(n) {
@@ -883,35 +845,14 @@ void computeAlignments(shb_context* c, const void* candidatesHost, uint64_t n, c
         if(call.error) std::rethrow_exception(call.error);
     }
 
-    // ---- results: the segments were rebased, digested and (in the steady state) copied to the host in candidate order while
-    // the later batches were still running (finaliseReadySegments); what is left is whatever could not be copied early.
-    SHB_CUDA(cudaStreamSynchronize(call.finalStream));
-    const uint64_t count = call.outCount, outBytes = call.outBytes;
+    // ---- results: the segments were rebased, digested and copied to the host in candidate order while the later batches were
+    // still running (finaliseReadySegments); what is left is the copy of the last ones.
     const auto copy0 = std::chrono::steady_clock::now();
+    SHB_CUDA(cudaStreamSynchronize(call.finalStream));
+    copier.finish();
+    const uint64_t count = call.outCount, outBytes = call.outBytes;
     SHB_REQUIRE(call.nextToFinalise == call.ledger.size() && call.finalRecords == count && call.finalBytes == outBytes, SHB_ERR_CUDA,
                 "Internal error: not every batch was finalised.");
-    const bool earlyCopy = call.hostRecords != nullptr;
-    if(!earlyCopy) {        // first call (no page-locked result blocks yet): exact-size buffers, pipelined copy through pinned staging
-        recOut.reset(allocHostResult(64 * count)); tocOut.reset(allocHostResult(8 * (count + 1)));
-    }
-    if(!earlyCopy || call.dataOverflow) dataOut.reset(allocHostResult(outBytes));
-    SHB_REQUIRE(recOut.p && tocOut.p && dataOut.p, SHB_ERR_OOM, "Out of host memory for the alignments.");
-    if(count && (!earlyCopy || call.dataOverflow)) {
-        const bool lockedRec = HostPool::instance().isPageLocked(recOut.p), lockedToc = HostPool::instance().isPageLocked(tocOut.p),
-                   lockedData = HostPool::instance().isPageLocked(dataOut.p);
-        uint64_t finalRecords = 0, finalBytes = 0;
-        for(const auto& entry : call.ledger) {
-            const AlignCall::Segment& seg = entry.second;
-            if(!seg.kept) continue;
-            if(!earlyCopy) {
-                copyToHostPipelined(c, static_cast<uint8_t*>(recOut.p) + 64 * finalRecords, ac.outRecords.get() + 16 * seg.recordBase, 64 * seg.kept, lockedRec);
-                copyToHostPipelined(c, static_cast<uint8_t*>(tocOut.p) + 8 * finalRecords, ac.outToc.get() + seg.recordBase, 8 * seg.kept, lockedToc);
-            }
-            copyToHostPipelined(c, static_cast<uint8_t*>(dataOut.p) + finalBytes, ac.outData.get() + seg.byteBase, seg.bytes, lockedData);
-            finalRecords += seg.kept; finalBytes += seg.bytes;
-        }
-        SHB_CUDA(cudaStreamSynchronize(st));
-    }
     if(n) ac.lastBytesPerCandidate = double(outBytes) / double(n);
     unsigned long long* digests = call.digests;
     // Counters of the workers.
@@ -928,7 +869,7 @@ void computeAlignments(shb_context* c, const void* candidatesHost, uint64_t n, c
     }
     SHB_CUDA(cudaMemcpyAsync(digestHost, digests, sizeof(digestHost), cudaMemcpyDeviceToHost, st));
     SHB_CUDA(cudaStreamSynchronize(st));
-    uint64_t* tocHostOut = static_cast<uint64_t*>(tocOut.p);
+    uint64_t* tocHostOut = reinterpret_cast<uint64_t*>(tocOut.data());
     tocHostOut[count] = outBytes;
     if(count == 0) tocHostOut[0] = 0;
     totalTimer.stop(st);
@@ -950,8 +891,8 @@ void computeAlignments(shb_context* c, const void* candidatesHost, uint64_t n, c
         result->outputCopyMs = msSince(copy0);
         result->hostWallMs = msSince(wall0);
     }
-    *alignmentDataOut = recOut.take(); *alignmentCountOut = count;
-    *compressedTocOut = static_cast<uint64_t*>(tocOut.take()); *compressedDataOut = static_cast<uint8_t*>(dataOut.take());
+    *alignmentDataOut = recOut.owner.take(); *alignmentCountOut = count;
+    *compressedTocOut = static_cast<uint64_t*>(tocOut.owner.take()); *compressedDataOut = static_cast<uint8_t*>(dataOut.owner.take());
 }
 
 } // namespace shb

@@ -142,7 +142,7 @@ void shb_context_destroy(shb_context* c)
     destroyDistState(c);
     destroyAlignCache(c);
     destroyLowhashState(c);
-    for(int i = 0; i < 2; i++) { if(c->pinnedStage[i]) cudaFreeHost(c->pinnedStage[i]); if(c->stageEvent[i]) cudaEventDestroy(c->stageEvent[i]); }
+    for(int i = 0; i < shb::kStageSlots; i++) { if(c->pinnedStage[i]) cudaFreeHost(c->pinnedStage[i]); if(c->stageEvent[i]) cudaEventDestroy(c->stageEvent[i]); }
     if(c->stream) cudaStreamDestroy(c->stream);
     for(int i = 0; i < 2; i++) if(c->copyStream[i]) cudaStreamDestroy(c->copyStream[i]);
     delete c;

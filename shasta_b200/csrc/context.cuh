@@ -18,6 +18,8 @@ inline uint32_t envCount(const char* name, uint32_t dflt)
 }
 
 constexpr int kMaxFusedIterations = 16;         // LowHash iterations hashed per pass over the k-mer ids (one slab each)
+constexpr int kStageSlots = 8;                  // pinned staging chunks of the device -> host result copies (hostcopy.cuh)
+constexpr uint64_t kStageBytes = 8ull << 20;
 
 // The words of shb_context::scalars, the context's small device scratch for totals and counters. Every stage has slots of
 // its own, so no two stages share a word whatever the order of the calls. The uint32 totals use the low half of their word.
@@ -117,8 +119,8 @@ struct shb_context {
 
     shb::DeviceBuffer<uint64_t> partKeys; shb::DeviceBuffer<uint32_t> partVals;
     void* lowhashState = nullptr;
-    void* pinnedStage[2] = {nullptr, nullptr};      // pinned staging for pipelined device->host result copies
-    cudaEvent_t stageEvent[2] = {nullptr, nullptr};
+    void* pinnedStage[shb::kStageSlots] = {};       // pinned staging ring of the device -> host result copies (hostcopy.cuh)
+    cudaEvent_t stageEvent[shb::kStageSlots] = {};
 
     // ---- alignment cache (downsampled markers; see align.cu) ------------------------------------
     void* alignCache = nullptr;

@@ -3,7 +3,7 @@
 // see DESIGN.md for the data layout and the per-kernel roofline.
 #include "context.cuh"
 #include "lowhash_kernels.cuh"
-#include "hostpool.cuh"
+#include "hostcopy.cuh"
 #include "digest.cuh"
 
 #include <algorithm>
@@ -480,14 +480,18 @@ void lowhashEmit(shb_context* c, void** candidatesOut, uint64_t* candidateCountO
     LowHashState& S = lowhashState(c);
     const uint64_t nOut = lowhashEmitDevice(c);
     cudaStream_t st = c->stream;
-    HostResult host(allocHostResult(nOut * 12));
-    SHB_REQUIRE(host.p != nullptr, SHB_ERR_OOM, "Out of host memory for the alignment candidates.");
+    HostBlock host(nOut * 12);
     unsigned long long digest = 0;
-    if(nOut) SHB_CUDA(cudaMemcpyAsync(host.p, c->candidatesDev.get(), nOut * 12, cudaMemcpyDeviceToHost, st));
-    SHB_CUDA(cudaMemcpyAsync(&digest, c->scalar(kSlotCandidateDigest), sizeof(digest), cudaMemcpyDeviceToHost, st));
-    SHB_CUDA(cudaStreamSynchronize(st));
+    {
+        // direct DMA into a page-locked block; into a pageable one through the staging ring, on three copier threads
+        StagedCopier copier(c, st, 3);
+        copyResult(copier, st, host, 0, reinterpret_cast<const uint8_t*>(c->candidatesDev.get()), nOut * 12);
+        SHB_CUDA(cudaMemcpyAsync(&digest, c->scalar(kSlotCandidateDigest), sizeof(digest), cudaMemcpyDeviceToHost, st));
+        SHB_CUDA(cudaStreamSynchronize(st));
+        copier.finish();
+    }
     S.candidateDigest = digest;
-    *candidatesOut = host.take();
+    *candidatesOut = host.owner.take();
     *candidateCountOut = nOut;
 }
 
