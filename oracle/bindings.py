@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE — ctypes bindings to the CPU oracle (oracle/_build/liboracle.so) and,
-when present, to the unmodified reference build (oracle/_ref/libshasta_ref.so).
+when present, to the unmodified reference build (oracle/_ref/libshasta_ref.so), both built by oracle/Makefile.
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may
 import this module. The product (shasta_b200/) never does.
@@ -12,48 +12,116 @@ import subprocess
 
 import numpy as np
 
+from oracle._load import have, load, take
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 ORACLE_SO = os.path.join(_HERE, "_build", "liboracle.so")
 REF_SO = os.path.join(_HERE, "_ref", "libshasta_ref.so")
 
 
 def build(quiet=True):
-    """Compile the oracle (always) and the reference build (only where the Makefile's SHASTA_REF_SRC tree exists)."""
-    out = subprocess.DEVNULL if quiet else None
-    subprocess.check_call(["make", "-C", _HERE, "oracle"], stdout=out)
-    subprocess.check_call(["make", "-C", _HERE, "-j8", "ref"], stdout=out)
+    """Compile the oracle (always) and every reference library (only where the Makefile's SHASTA_REF_SRC tree exists)."""
+    subprocess.check_call(["make", "-C", _HERE, "-j8", "all"], stdout=subprocess.DEVNULL if quiet else None)
 
 
-_oracle = None
-_ref = None
+class AlignOptions(C.Structure):
+    """orc_align_options: AlignOptions of src/AssemblerOptions.hpp:177-199 as used on the path."""
+    _fields_ = [("alignMethod", C.c_uint32), ("k", C.c_uint32),
+                ("maxSkip", C.c_uint64), ("maxDrift", C.c_uint64), ("maxTrim", C.c_uint64),
+                ("minAlignedMarkerCount", C.c_uint64), ("minAlignedFraction", C.c_double),
+                ("matchScore", C.c_int32), ("mismatchScore", C.c_int32), ("gapScore", C.c_int32),
+                ("downsamplingFactor", C.c_double), ("bandExtend", C.c_int32), ("maxBand", C.c_int32),
+                ("suppressContainments", C.c_uint32),
+                ("align4DeltaX", C.c_uint64), ("align4DeltaY", C.c_uint64),
+                ("align4MinEntryCountPerCell", C.c_uint64), ("align4MaxDistanceFromBoundary", C.c_uint64)]
 
 
-def oracle_lib():
-    global _oracle
-    if _oracle is None:
-        if not os.path.exists(ORACLE_SO):
-            build()
-        _oracle = C.CDLL(ORACLE_SO)
-        _oracle.orc_murmurhash64a.restype = C.c_uint64
-        _oracle.orc_murmurhash64a.argtypes = [C.c_void_p, C.c_int, C.c_uint64]
-        _oracle.orc_murmurhash2.restype = C.c_uint32
-        _oracle.orc_murmurhash2.argtypes = [C.c_void_p, C.c_int, C.c_uint32]
-        _oracle.orc_reverse_complement_kmer.restype = C.c_uint32
-        _oracle.orc_reverse_complement_kmer.argtypes = [C.c_uint32, C.c_uint32]
-        _oracle.orc_kmer_downsampling_hash.restype = C.c_uint32
-        _oracle.orc_kmer_downsampling_hash.argtypes = [C.c_uint32, C.c_uint32]
-        _oracle.orc_lowhash0.restype = C.c_int
-        _oracle.orc_lowhash0.argtypes = [
-            C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
-            C.c_uint64, C.c_double, C.c_uint64, C.c_double, C.c_uint64,
-            C.c_uint64, C.c_uint64, C.c_uint64,
-            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
-        _oracle.orc_free.argtypes = [C.c_void_p]
-    return _oracle
+class _Alignment(C.Structure):
+    _fields_ = [("ord", C.c_void_p), ("n", C.c_uint64), ("cap", C.c_uint64)]
+
+
+_TABLE = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]
+_READ_GRAPH = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+_READ_GRAPH2 = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32] + [C.c_void_p] * 7
+_HISTOGRAM2 = [C.c_void_p, C.c_uint64, C.c_double, C.c_double, C.c_uint64, C.c_double]
+
+_ORACLE_PROTOS = {
+    "orc_murmurhash64a": (C.c_uint64, [C.c_void_p, C.c_int, C.c_uint64]),
+    "orc_murmurhash2": (C.c_uint32, [C.c_void_p, C.c_int, C.c_uint32]),
+    "orc_reverse_complement_kmer": (C.c_uint32, [C.c_uint32, C.c_uint32]),
+    "orc_kmer_downsampling_hash": (C.c_uint32, [C.c_uint32, C.c_uint32]),
+    "orc_lowhash0": (C.c_int, [C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.c_uint64, C.c_double, C.c_uint64, C.c_double, C.c_uint64,
+                               C.c_uint64, C.c_uint64, C.c_uint64,
+                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]),
+    "orc_free": (None, [C.c_void_p]),
+    "orc_find_markers": (C.c_int, [C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_void_p]),
+    "orc_overlap_align": (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
+                                    C.c_int64, C.c_int64, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]),
+    "orc_compress_alignment": (C.c_uint64, [C.c_void_p, C.c_uint64, C.c_void_p]),
+    "orc_decompress_alignment": (C.c_uint64, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]),
+    "orc_alignment_info": (None, [C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p]),
+    "orc_align_method3": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(AlignOptions), C.c_void_p]),
+    "orc_align_method4": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(AlignOptions), C.c_void_p,
+                                    C.POINTER(C.c_int)]),
+    "orc_compute_alignments": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(AlignOptions), C.c_uint32,
+                                         C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(C.c_void_p),
+                                         C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),
+    "orc_compute_alignment_table": (None, _TABLE),
+    "orc_compute_candidate_table": (None, _TABLE),
+    "orc_create_read_graph": (C.c_int, _READ_GRAPH),
+    "orc_create_read_graph2": (C.c_int, _READ_GRAPH2),
+    "orc_histogram2_threshold": (C.c_double, _HISTOGRAM2),
+    "orc_set_dp_policy": (None, [C.c_int]),
+    "orc_get_dp_policy": (C.c_int, []),
+    "orc_reset_tie_flags": (None, []),
+    "orc_get_tie_flags": (C.c_int, []),
+    "orc_release_thread_scratch": (None, []),
+}
+
+_REF_PROTOS = {
+    "ref_lowhash0": (C.c_int, [C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.c_uint64, C.c_double, C.c_uint64, C.c_double, C.c_uint64,
+                               C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
+                               C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                               C.c_void_p, C.c_uint64, C.c_void_p]),
+    "ref_markers_from_fasta": (C.c_int, [C.c_char_p, C.c_uint64, C.c_double, C.c_int, C.c_uint64, C.c_uint64,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ref_reads_from_fasta": (C.c_int, [C.c_char_p, C.c_uint64, C.c_double, C.c_int, C.c_uint64, C.c_uint64,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "ref_murmurhash64a": (C.c_uint64, [C.c_void_p, C.c_int, C.c_uint64]),
+    "ref_murmurhash2": (C.c_uint32, [C.c_void_p, C.c_int, C.c_uint32]),
+    "ref_free": (None, [C.c_void_p]),
+    "ref_write_data_dir": (C.c_int, [C.c_char_p, C.c_char_p, C.c_uint64, C.c_double, C.c_int, C.c_uint64, C.c_uint64]),
+    "ref_open_vector": (C.c_int, [C.c_char_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]),
+    "ref_align4": (C.c_int, [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
+                             C.c_uint64, C.c_double, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
+                             C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]),
+    "ref_alignment_info": (None, [C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p]),
+    "ref_compress_alignment": (C.c_uint64, [C.c_void_p, C.c_uint64, C.c_void_p]),
+    "ref_decompress_alignment": (C.c_uint64, [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]),
+    "ref_test_alignment_compression": (C.c_int, []),
+    "ref_histogram2_threshold": (C.c_double, _HISTOGRAM2),
+    "ref_alignment_indicators": (None, [C.c_void_p, C.c_void_p]),
+    "ref_compute_alignment_table": (C.c_int, _TABLE),
+    "ref_compute_candidate_table": (C.c_int, _TABLE),
+    "ref_create_read_graph": (C.c_int, _READ_GRAPH),
+    "ref_create_read_graph2": (C.c_int, _READ_GRAPH2),
+}
+
+
+def oracle_lib(protos=None):
+    """liboracle.so, built first if it is missing, with this module's prototypes and, when given, those of protos: the table
+    of the binding module that wraps the restatements it calls."""
+    if not os.path.exists(ORACLE_SO):
+        build()
+    lib = load(ORACLE_SO, _ORACLE_PROTOS)
+    return load(ORACLE_SO, protos) if protos else lib
 
 
 def have_ref():
-    return os.path.exists(REF_SO)
+    return have(REF_SO)
 
 
 def have_ref_readgraph():
@@ -67,26 +135,7 @@ def have_ref_readgraph():
 
 
 def ref_lib():
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_SO)
-        _ref.ref_lowhash0.restype = C.c_int
-        _ref.ref_lowhash0.argtypes = [
-            C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p,
-            C.c_uint64, C.c_double, C.c_uint64, C.c_double, C.c_uint64,
-            C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
-            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
-            C.c_void_p, C.c_uint64, C.c_void_p]
-        _ref.ref_markers_from_fasta.restype = C.c_int
-        _ref.ref_markers_from_fasta.argtypes = [
-            C.c_char_p, C.c_uint64, C.c_double, C.c_int, C.c_uint64, C.c_uint64,
-            C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        _ref.ref_murmurhash64a.restype = C.c_uint64
-        _ref.ref_murmurhash64a.argtypes = [C.c_void_p, C.c_int, C.c_uint64]
-        _ref.ref_murmurhash2.restype = C.c_uint32
-        _ref.ref_murmurhash2.argtypes = [C.c_void_p, C.c_int, C.c_uint32]
-        _ref.ref_free.argtypes = [C.c_void_p]
-    return _ref
+    return load(REF_SO, _REF_PROTOS)
 
 
 class LowHashParams(dict):
@@ -132,9 +181,7 @@ def oracle_lowhash0(toc, data, flags, p: LowHashParams, max_iters=4096):
         raise RuntimeError("alignmentCandidatesPerRead was not reached within max_iters iterations")
     if rc != 0:
         raise RuntimeError("log2MinHashBucketCount is unreasonably small.")
-    out = np.ctypeslib.as_array(C.cast(cand, C.POINTER(C.c_uint32)), (n.value, 3)).copy() if n.value else np.zeros((0, 3), np.uint32)
-    lib.orc_free(cand)
-    return out, stats, summ[:iters.value].copy()
+    return take(cand, 3 * n.value, np.uint32, lib.orc_free).reshape(-1, 3), stats, summ[:iters.value].copy()
 
 
 def ref_lowhash0(toc, data, flags, p: LowHashParams, threads=0, max_iters=4096, quiet=True):
@@ -155,9 +202,7 @@ def ref_lowhash0(toc, data, flags, p: LowHashParams, threads=0, max_iters=4096, 
                           summ.ctypes.data, max_iters, C.byref(iters))
     if rc != 0:
         raise RuntimeError("reference LowHash0 failed")
-    out = np.ctypeslib.as_array(C.cast(cand, C.POINTER(C.c_uint32)), (n.value, 3)).copy() if n.value else np.zeros((0, 3), np.uint32)
-    lib.ref_free(cand)
-    return out, stats, summ[:iters.value].copy(), sec.value
+    return take(cand, 3 * n.value, np.uint32, lib.ref_free).reshape(-1, 3), stats, summ[:iters.value].copy(), sec.value
 
 
 def ref_markers_from_fasta(path, k=10, probability=0.1, seed=231, min_read_length=10000, threads=4, want_hash=False):
@@ -173,16 +218,11 @@ def ref_markers_from_fasta(path, k=10, probability=0.1, seed=231, min_read_lengt
     if rc != 0:
         raise RuntimeError("reference marker finding failed")
     R = R.value
-    tocn = np.ctypeslib.as_array(C.cast(toc, C.POINTER(C.c_uint64)), (2 * R + 1,)).copy()
-    M = int(tocn[-1])
-    datan = np.ctypeslib.as_array(C.cast(data, C.POINTER(C.c_uint8)), (M * 7,)).copy()
-    flagsn = np.ctypeslib.as_array(C.cast(flags, C.POINTER(C.c_uint8)), (R,)).copy()
-    out = dict(toc=tocn, data=datan, flags=flagsn, k=k)
+    tocn = take(toc, 2 * R + 1, np.uint64, lib.ref_free)
+    out = dict(toc=tocn, data=take(data, 7 * int(tocn[-1]), np.uint8, lib.ref_free), flags=take(flags, R, np.uint8, lib.ref_free),
+               k=k)
     if want_hash:
-        out["kmerHash"] = np.ctypeslib.as_array(C.cast(kh, C.POINTER(C.c_uint32)), (1 << (2 * k),)).copy()
-        lib.ref_free(kh)
-    for ptr in (toc, data, flags):
-        lib.ref_free(ptr)
+        out["kmerHash"] = take(kh, 1 << (2 * k), np.uint32, lib.ref_free)
     return out
 
 
@@ -190,9 +230,6 @@ def ref_reads_from_fasta(path, k=10, probability=0.1, seed=231, min_read_length=
     """The inputs of the reference's MarkerFinder as the reference stores them: dict(word_offsets uint64[R+1], words uint64[],
     base_counts uint64[R], is_marker uint8[4^k]) — RLE reads in LongBaseSequences layout + kmerTable[].isMarker."""
     lib = ref_lib()
-    lib.ref_reads_from_fasta.restype = C.c_int
-    lib.ref_reads_from_fasta.argtypes = [C.c_char_p, C.c_uint64, C.c_double, C.c_int, C.c_uint64, C.c_uint64,
-                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     R = C.c_uint64()
     off, words, bc, im = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
     rc = lib.ref_reads_from_fasta(path.encode(), k, probability, seed, min_read_length, threads,
@@ -200,22 +237,14 @@ def ref_reads_from_fasta(path, k=10, probability=0.1, seed=231, min_read_length=
     if rc != 0:
         raise RuntimeError("reference read loading failed")
     R = R.value
-    offn = np.ctypeslib.as_array(C.cast(off, C.POINTER(C.c_uint64)), (R + 1,)).copy()
-    n = int(offn[-1])
-    out = dict(word_offsets=offn,
-               words=np.ctypeslib.as_array(C.cast(words, C.POINTER(C.c_uint64)), (n,)).copy() if n else np.zeros(0, np.uint64),
-               base_counts=np.ctypeslib.as_array(C.cast(bc, C.POINTER(C.c_uint64)), (R,)).copy() if R else np.zeros(0, np.uint64),
-               is_marker=np.ctypeslib.as_array(C.cast(im, C.POINTER(C.c_uint8)), (1 << (2 * k),)).copy(), k=k)
-    for ptr in (off, words, bc, im):
-        lib.ref_free(ptr)
-    return out
+    offn = take(off, R + 1, np.uint64, lib.ref_free)
+    return dict(word_offsets=offn, words=take(words, int(offn[-1]), np.uint64, lib.ref_free),
+                base_counts=take(bc, R, np.uint64, lib.ref_free), is_marker=take(im, 1 << (2 * k), np.uint8, lib.ref_free), k=k)
 
 
 def oracle_find_markers(word_offsets, words, base_counts, is_marker, k):
     """CPU restatement of MarkerFinder (oracle/markers_oracle.c). Returns (toc uint64[2R+1], data uint8[7M])."""
     lib = oracle_lib()
-    lib.orc_find_markers.restype = C.c_int
-    lib.orc_find_markers.argtypes = [C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     wo = np.ascontiguousarray(word_offsets, np.uint64)
     w = np.ascontiguousarray(words, np.uint64)
     bc = np.ascontiguousarray(base_counts, np.uint64)
@@ -223,12 +252,8 @@ def oracle_find_markers(word_offsets, words, base_counts, is_marker, k):
     R = len(bc)
     toc, data = C.c_void_p(), C.c_void_p()
     lib.orc_find_markers(R, k, wo.ctypes.data, w.ctypes.data, bc.ctypes.data, im.ctypes.data, C.byref(toc), C.byref(data))
-    tocn = np.ctypeslib.as_array(C.cast(toc, C.POINTER(C.c_uint64)), (2 * R + 1,)).copy()
-    M = int(tocn[-1])
-    datan = np.ctypeslib.as_array(C.cast(data, C.POINTER(C.c_uint8)), (7 * M,)).copy() if M else np.zeros(0, np.uint8)
-    lib.orc_free(toc)
-    lib.orc_free(data)
-    return tocn, datan
+    tocn = take(toc, 2 * R + 1, np.uint64, lib.orc_free)
+    return tocn, take(data, 7 * int(tocn[-1]), np.uint8, lib.orc_free)
 
 
 def candidate_digest(c):
@@ -242,18 +267,6 @@ def candidate_digest(c):
 
 # ---------------------------------------------------------------------------------------------------
 # Alignment half
-class AlignOptions(C.Structure):
-    """orc_align_options: AlignOptions of src/AssemblerOptions.hpp:177-199 as used on the path."""
-    _fields_ = [("alignMethod", C.c_uint32), ("k", C.c_uint32),
-                ("maxSkip", C.c_uint64), ("maxDrift", C.c_uint64), ("maxTrim", C.c_uint64),
-                ("minAlignedMarkerCount", C.c_uint64), ("minAlignedFraction", C.c_double),
-                ("matchScore", C.c_int32), ("mismatchScore", C.c_int32), ("gapScore", C.c_int32),
-                ("downsamplingFactor", C.c_double), ("bandExtend", C.c_int32), ("maxBand", C.c_int32),
-                ("suppressContainments", C.c_uint32),
-                ("align4DeltaX", C.c_uint64), ("align4DeltaY", C.c_uint64),
-                ("align4MinEntryCountPerCell", C.c_uint64), ("align4MaxDistanceFromBoundary", C.c_uint64)]
-
-
 ALIGN_DEFAULTS = dict(alignMethod=3, k=10, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=100,
                       minAlignedFraction=0.4, matchScore=6, mismatchScore=-1, gapScore=-1, downsamplingFactor=0.1,
                       bandExtend=10, maxBand=1000, suppressContainments=0, align4DeltaX=200, align4DeltaY=10,
@@ -266,40 +279,9 @@ def make_align_options(**kw):
     return AlignOptions(**d)
 
 
-def _align_protos(lib):
-    lib.orc_overlap_align.restype = C.c_int
-    lib.orc_overlap_align.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int,
-                                      C.c_int64, C.c_int64, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
-    lib.orc_compress_alignment.restype = C.c_uint64
-    lib.orc_compress_alignment.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p]
-    lib.orc_decompress_alignment.restype = C.c_uint64
-    lib.orc_decompress_alignment.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
-    lib.orc_alignment_info.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p]
-    lib.orc_align_method3.restype = C.c_int
-    lib.orc_align_method3.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(AlignOptions), C.c_void_p]
-    lib.orc_align_method4.restype = C.c_int
-    lib.orc_align_method4.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(AlignOptions), C.c_void_p, C.POINTER(C.c_int)]
-    lib.orc_compute_alignments.restype = C.c_int
-    lib.orc_compute_alignments.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.POINTER(AlignOptions), C.c_uint32,
-                                           C.POINTER(C.c_void_p), C.POINTER(C.c_uint64), C.POINTER(C.c_void_p),
-                                           C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-
-
-class _Alignment(C.Structure):
-    _fields_ = [("ord", C.c_void_p), ("n", C.c_uint64), ("cap", C.c_uint64)]
-
-
-def _olib():
-    lib = oracle_lib()
-    if not getattr(lib, "_align_ready", False):
-        _align_protos(lib)
-        lib._align_ready = True
-    return lib
-
-
 def overlap_align(a, b, match=6, mismatch=-1, gap=-1, band=None):
     """The oracle's DP. Returns (score, path uint32[n,2]) — diagonal steps in path order; score None on failure."""
-    lib = _olib()
+    lib = oracle_lib()
     a = np.ascontiguousarray(a, np.uint32)
     b = np.ascontiguousarray(b, np.uint32)
     p = C.c_void_p()
@@ -309,21 +291,12 @@ def overlap_align(a, b, match=6, mismatch=-1, gap=-1, band=None):
                               1 if band is not None else 0, lo, hi, C.byref(p), C.byref(n))
     if s == -2**31:
         return None, np.zeros((0, 2), np.uint32)
-    path = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint32)), (n.value, 2)).copy() if n.value else np.zeros((0, 2), np.uint32)
-    lib.orc_free(p)
-    return s, path
-
-
-def _take_alignment(lib, al):
-    out = np.ctypeslib.as_array(C.cast(al.ord, C.POINTER(C.c_uint32)), (al.n, 2)).copy() if al.n else np.zeros((0, 2), np.uint32)
-    if al.ord:
-        lib.orc_free(al.ord)
-    return out
+    return s, take(p, 2 * n.value, np.uint32, lib.orc_free).reshape(-1, 2)
 
 
 def oracle_align_pair(a, b, opts: AlignOptions):
     """Single pair through method 3 or 4. Returns (status, ordinals uint32[n,2], tie flag)."""
-    lib = _olib()
+    lib = oracle_lib()
     a = np.ascontiguousarray(a, np.uint32)
     b = np.ascontiguousarray(b, np.uint32)
     al = _Alignment(None, 0, 0)
@@ -332,11 +305,11 @@ def oracle_align_pair(a, b, opts: AlignOptions):
         st = lib.orc_align_method4(a.ctypes.data, len(a), b.ctypes.data, len(b), C.byref(opts), C.byref(al), C.byref(tie))
     else:
         st = lib.orc_align_method3(a.ctypes.data, len(a), b.ctypes.data, len(b), C.byref(opts), C.byref(al))
-    return st, _take_alignment(lib, al), tie.value
+    return st, take(al.ord, 2 * al.n, np.uint32, lib.orc_free).reshape(-1, 2), tie.value
 
 
 def oracle_alignment_info(ordinals, nx, ny):
-    lib = _olib()
+    lib = oracle_lib()
     o = np.ascontiguousarray(ordinals, np.uint32).reshape(-1)
     out = np.zeros(12, np.uint32)
     lib.orc_alignment_info(o.ctypes.data, len(o) // 2, nx, ny, out.ctypes.data)
@@ -344,7 +317,7 @@ def oracle_alignment_info(ordinals, nx, ny):
 
 
 def oracle_compress(ordinals):
-    lib = _olib()
+    lib = oracle_lib()
     o = np.ascontiguousarray(ordinals, np.uint32).reshape(-1)
     buf = np.zeros(8 * len(o) + 16, np.uint8)
     n = lib.orc_compress_alignment(o.ctypes.data, len(o) // 2, buf.ctypes.data)
@@ -352,7 +325,7 @@ def oracle_compress(ordinals):
 
 
 def oracle_decompress(data, cap=1 << 20):
-    lib = _olib()
+    lib = oracle_lib()
     d = np.ascontiguousarray(data, np.uint8)
     out = np.zeros((cap, 2), np.uint32)
     n = lib.orc_decompress_alignment(d.ctypes.data, len(d), out.ctypes.data, cap)
@@ -361,7 +334,7 @@ def oracle_decompress(data, cap=1 << 20):
 
 def oracle_compute_alignments(toc, kmer_ids, candidates, opts: AlignOptions, threads=1):
     """Returns (records uint32[count,16], compressedToc uint64[count+1], compressedData uint8[], ties uint8[n])."""
-    lib = _olib()
+    lib = oracle_lib()
     toc = np.ascontiguousarray(toc, np.uint64)
     kmer_ids = np.ascontiguousarray(kmer_ids, np.uint32)
     cand = np.ascontiguousarray(candidates, np.uint32).reshape(-1, 3)
@@ -373,36 +346,14 @@ def oracle_compute_alignments(toc, kmer_ids, candidates, opts: AlignOptions, thr
     lib.orc_compute_alignments(toc.ctypes.data, kmer_ids.ctypes.data, cand.ctypes.data, len(cand), C.byref(opts), threads,
                                C.byref(rec), C.byref(cnt), C.byref(ctoc), C.byref(cdata), C.byref(ties))
     n = cnt.value
-    records = np.ctypeslib.as_array(C.cast(rec, C.POINTER(C.c_uint32)), (n, 16)).copy() if n else np.zeros((0, 16), np.uint32)
-    ctocn = np.ctypeslib.as_array(C.cast(ctoc, C.POINTER(C.c_uint64)), (n + 1,)).copy()
-    nb = int(ctocn[-1])
-    cdatan = np.ctypeslib.as_array(C.cast(cdata, C.POINTER(C.c_uint8)), (nb,)).copy() if nb else np.zeros(0, np.uint8)
-    tiesn = np.ctypeslib.as_array(C.cast(ties, C.POINTER(C.c_uint8)), (len(cand),)).copy() if len(cand) else np.zeros(0, np.uint8)
-    for p in (rec, ctoc, cdata, ties):
-        lib.orc_free(p)
-    return records, ctocn, cdatan, tiesn
+    records = take(rec, 16 * n, np.uint32, lib.orc_free).reshape(-1, 16)
+    ctocn = take(ctoc, n + 1, np.uint64, lib.orc_free)
+    return records, ctocn, take(cdata, int(ctocn[-1]), np.uint8, lib.orc_free), take(ties, len(cand), np.uint8, lib.orc_free)
 
 
 # ---- reference side (unmodified Align4.cpp / Alignment.cpp / compressAlignment.cpp) ----
-def _rlib():
-    lib = ref_lib()
-    if not getattr(lib, "_align_ready", False):
-        lib.ref_align4.restype = C.c_int
-        lib.ref_align4.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
-                                   C.c_uint64, C.c_double, C.c_uint64, C.c_uint64, C.c_uint64, C.c_uint64,
-                                   C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
-        lib.ref_alignment_info.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p]
-        lib.ref_compress_alignment.restype = C.c_uint64
-        lib.ref_compress_alignment.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p]
-        lib.ref_decompress_alignment.restype = C.c_uint64
-        lib.ref_decompress_alignment.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
-        lib.ref_test_alignment_compression.restype = C.c_int
-        lib._align_ready = True
-    return lib
-
-
 def ref_align4(a, b, opts: AlignOptions):
-    lib = _rlib()
+    lib = ref_lib()
     a = np.ascontiguousarray(a, np.uint32)
     b = np.ascontiguousarray(b, np.uint32)
     p = C.c_void_p()
@@ -412,13 +363,11 @@ def ref_align4(a, b, opts: AlignOptions):
                         opts.minAlignedFraction, opts.maxSkip, opts.maxDrift, opts.maxTrim, opts.maxBand, C.byref(p), C.byref(n))
     if rc:
         raise RuntimeError("reference Align4 failed")
-    out = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint32)), (n.value, 2)).copy() if n.value else np.zeros((0, 2), np.uint32)
-    lib.ref_free(p)
-    return out
+    return take(p, 2 * n.value, np.uint32, lib.ref_free).reshape(-1, 2)
 
 
 def ref_alignment_info(ordinals, nx, ny):
-    lib = _rlib()
+    lib = ref_lib()
     o = np.ascontiguousarray(ordinals, np.uint32).reshape(-1)
     out = np.zeros(12, np.uint32)
     lib.ref_alignment_info(o.ctypes.data, len(o) // 2, nx, ny, out.ctypes.data)
@@ -426,7 +375,7 @@ def ref_alignment_info(ordinals, nx, ny):
 
 
 def ref_compress(ordinals):
-    lib = _rlib()
+    lib = ref_lib()
     o = np.ascontiguousarray(ordinals, np.uint32).reshape(-1)
     buf = np.zeros(8 * len(o) + 16, np.uint8)
     n = lib.ref_compress_alignment(o.ctypes.data, len(o) // 2, buf.ctypes.data)
@@ -435,22 +384,20 @@ def ref_compress(ordinals):
 
 def oracle_compute_alignment_table(records, read_count):
     """Returns (toc uint32[2R+1], table uint32[4n]) — src/AssemblerAlign.cpp:509-571."""
-    lib = _olib()
+    lib = oracle_lib()
     rec = np.ascontiguousarray(records, np.uint32).reshape(-1, 16)
     toc = np.zeros(2 * read_count + 1, np.uint32)
     table = np.zeros(4 * len(rec) + 1, np.uint32)
-    lib.orc_compute_alignment_table.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]
     lib.orc_compute_alignment_table(rec.ctypes.data, len(rec), read_count, toc.ctypes.data, table.ctypes.data)
     return toc, table[:4 * len(rec)].copy()
 
 
 def oracle_compute_candidate_table(candidates, read_count):
     """Returns (toc uint64[2R+1], table uint64[4n]) — src/AssemblerAlignmentCandidates.cpp:379-448."""
-    lib = _olib()
+    lib = oracle_lib()
     cand = np.ascontiguousarray(candidates, np.uint32).reshape(-1, 3)
     toc = np.zeros(2 * read_count + 1, np.uint64)
     table = np.zeros(4 * len(cand) + 1, np.uint64)
-    lib.orc_compute_candidate_table.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]
     lib.orc_compute_candidate_table(cand.ctypes.data, len(cand), read_count, toc.ctypes.data, table.ctypes.data)
     return toc, table[:4 * len(cand)].copy()
 
@@ -477,13 +424,10 @@ def oracle_create_read_graph(records, read_count, max_alignment_count):
     Returns (records with isInReadGraph set, keep uint8[n], edges uint32[E,4], connectivityToc uint32[2R+1], connectivityData uint32[2E]);
     each connectivity row lists its edges in decreasing edge index, as the reference's VectorOfVectors::store leaves them.
     Raises UnorderedReadGraphEdge where the reference's assertion fails."""
-    lib = _olib()
+    lib = oracle_lib()
     rec, keep, edges, toc, data = _read_graph_buffers(records, read_count)
     n = len(rec)
     e = C.c_uint64()
-    lib.orc_create_read_graph.restype = C.c_int
-    lib.orc_create_read_graph.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                          C.c_void_p]
     if lib.orc_create_read_graph(rec.ctypes.data, n, read_count, int(max_alignment_count), keep.ctypes.data, edges.ctypes.data,
                                  C.byref(e), toc.ctypes.data, data.ctypes.data):
         raise UnorderedReadGraphEdge("a kept alignment gives an unordered read graph edge")
@@ -495,15 +439,12 @@ def oracle_create_read_graph2(records, read_count, max_alignment_count, percenti
     """Assembler::createReadGraph2, creationMethod 2 (src/AssemblerReadGraph2.cpp:69-248). percentiles = (markerCount,
     alignedFraction, maxSkip, maxDrift, maxTrim). Returns (criteria dict, records, keep, edges, connectivityToc, connectivityData),
     the last five as in oracle_create_read_graph."""
-    lib = _olib()
+    lib = oracle_lib()
     rec, keep, edges, toc, data = _read_graph_buffers(records, read_count)
     n = len(rec)
     pc = np.array(percentiles, np.float64)
     crit = np.zeros(5, np.uint64)
     e = C.c_uint64()
-    lib.orc_create_read_graph2.restype = C.c_int
-    lib.orc_create_read_graph2.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                           C.c_void_p, C.c_void_p, C.c_void_p]
     if lib.orc_create_read_graph2(rec.ctypes.data, n, read_count, int(max_alignment_count), pc.ctypes.data, crit.ctypes.data,
                                   keep.ctypes.data, edges.ctypes.data, C.byref(e), toc.ctypes.data, data.ctypes.data):
         raise UnorderedReadGraphEdge("a kept alignment gives an unordered read graph edge")
@@ -514,13 +455,10 @@ def oracle_create_read_graph2(records, read_count, max_alignment_count, percenti
 def ref_create_read_graph(records, read_count, max_alignment_count):
     """The reference's createReadGraph and createReadGraphUsingSelectedAlignments over its own containers
     (oracle/ref_glue/ref_readgraph.cpp). Same arguments, returns and refusal as oracle_create_read_graph."""
-    lib = _rlib()
+    lib = ref_lib()
     rec, keep, edges, toc, data = _read_graph_buffers(records, read_count)
     n = len(rec)
     e = C.c_uint64()
-    lib.ref_create_read_graph.restype = C.c_int
-    lib.ref_create_read_graph.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                          C.c_void_p]
     if lib.ref_create_read_graph(rec.ctypes.data, n, read_count, int(max_alignment_count), keep.ctypes.data, edges.ctypes.data,
                                  C.byref(e), toc.ctypes.data, data.ctypes.data):
         raise UnorderedReadGraphEdge("the reference refused the read graph")
@@ -531,15 +469,12 @@ def ref_create_read_graph(records, read_count, max_alignment_count):
 def ref_create_read_graph2(records, read_count, max_alignment_count, percentiles):
     """The reference's createReadGraph2 (Histogram2 criteria, then the selection of createReadGraph) over its own containers.
     Same arguments, returns and refusal as oracle_create_read_graph2."""
-    lib = _rlib()
+    lib = ref_lib()
     rec, keep, edges, toc, data = _read_graph_buffers(records, read_count)
     n = len(rec)
     pc = np.array(percentiles, np.float64)
     crit = np.zeros(5, np.uint64)
     e = C.c_uint64()
-    lib.ref_create_read_graph2.restype = C.c_int
-    lib.ref_create_read_graph2.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                           C.c_void_p, C.c_void_p, C.c_void_p]
     if lib.ref_create_read_graph2(rec.ctypes.data, n, read_count, int(max_alignment_count), pc.ctypes.data, crit.ctypes.data,
                                   keep.ctypes.data, edges.ctypes.data, C.byref(e), toc.ctypes.data, data.ctypes.data):
         raise UnorderedReadGraphEdge("the reference refused the read graph")
@@ -549,12 +484,10 @@ def ref_create_read_graph2(records, read_count, max_alignment_count, percentiles
 
 def ref_compute_alignment_table(records, read_count):
     """The reference's computeAlignmentTable over its own VectorOfVectors. Returns (toc uint32[2R+1], table uint32[4n])."""
-    lib = _rlib()
+    lib = ref_lib()
     rec = np.ascontiguousarray(records, np.uint32).reshape(-1, 16)
     toc = np.zeros(2 * read_count + 1, np.uint32)
     table = np.zeros(4 * len(rec) + 1, np.uint32)
-    lib.ref_compute_alignment_table.restype = C.c_int
-    lib.ref_compute_alignment_table.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]
     if lib.ref_compute_alignment_table(rec.ctypes.data, len(rec), read_count, toc.ctypes.data, table.ctypes.data):
         raise RuntimeError("reference computeAlignmentTable failed")
     return toc, table[:4 * len(rec)].copy()
@@ -562,76 +495,55 @@ def ref_compute_alignment_table(records, read_count):
 
 def ref_compute_candidate_table(candidates, read_count):
     """The reference's computeCandidateTable over its own VectorOfVectors. Returns (toc uint64[2R+1], table uint64[4n])."""
-    lib = _rlib()
+    lib = ref_lib()
     cand = np.ascontiguousarray(candidates, np.uint32).reshape(-1, 3)
     toc = np.zeros(2 * read_count + 1, np.uint64)
     table = np.zeros(4 * len(cand) + 1, np.uint64)
-    lib.ref_compute_candidate_table.restype = C.c_int
-    lib.ref_compute_candidate_table.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_void_p]
     if lib.ref_compute_candidate_table(cand.ctypes.data, len(cand), read_count, toc.ctypes.data, table.ctypes.data):
         raise RuntimeError("reference computeCandidateTable failed")
     return toc, table[:4 * len(cand)].copy()
 
 
 def oracle_histogram2_threshold(x, start, stop, bin_count, fraction):
-    lib = _olib()
     x = np.ascontiguousarray(x, np.float64)
-    lib.orc_histogram2_threshold.restype = C.c_double
-    lib.orc_histogram2_threshold.argtypes = [C.c_void_p, C.c_uint64, C.c_double, C.c_double, C.c_uint64, C.c_double]
-    return lib.orc_histogram2_threshold(x.ctypes.data, len(x), start, stop, bin_count, fraction)
+    return oracle_lib().orc_histogram2_threshold(x.ctypes.data, len(x), start, stop, bin_count, fraction)
 
 
 def ref_histogram2_threshold(x, start, stop, bin_count, fraction):
     """The reference's own Histogram2 (dynamic bounds), compiled unmodified (oracle/_ref)."""
-    lib = _rlib()
     x = np.ascontiguousarray(x, np.float64)
-    lib.ref_histogram2_threshold.restype = C.c_double
-    lib.ref_histogram2_threshold.argtypes = [C.c_void_p, C.c_uint64, C.c_double, C.c_double, C.c_uint64, C.c_double]
-    return lib.ref_histogram2_threshold(x.ctypes.data, len(x), start, stop, bin_count, fraction)
+    return ref_lib().ref_histogram2_threshold(x.ctypes.data, len(x), start, stop, bin_count, fraction)
 
 
 def ref_alignment_indicators(record16):
     """(minAlignedFraction, markerCount, maxDrift, maxSkip, trim) by the reference's AlignmentInfo accessors."""
-    lib = _rlib()
     rec = np.ascontiguousarray(record16, np.uint32).reshape(16)
     out = np.zeros(5, np.float64)
-    lib.ref_alignment_indicators.argtypes = [C.c_void_p, C.c_void_p]
-    lib.ref_alignment_indicators(rec.ctypes.data, out.ctypes.data)
+    ref_lib().ref_alignment_indicators(rec.ctypes.data, out.ctypes.data)
     return out
 
 
 def set_dp_policy(bits):
     """Tie-break policy of the oracle's DP at run time (include/shb_dp_policy.h: bit 0 diagonal wins ties, bit 1 vertical
     before horizontal, bit 2 first maximum is the end cell). Returns the previous policy."""
-    lib = _olib()
-    lib.orc_get_dp_policy.restype = C.c_int
-    lib.orc_set_dp_policy.argtypes = [C.c_int]
+    lib = oracle_lib()
     old = lib.orc_get_dp_policy()
     lib.orc_set_dp_policy(int(bits))
     return old
 
 
 def default_dp_policy():
-    lib = _olib()
-    lib.orc_get_dp_policy.restype = C.c_int
-    return lib.orc_get_dp_policy()
+    return oracle_lib().orc_get_dp_policy()
 
 
 def ref_write_data_dir(fasta, prefix, k=10, probability=0.1, seed=231, min_read_length=10000, threads=4):
-    lib = ref_lib()
-    lib.ref_write_data_dir.restype = C.c_int
-    lib.ref_write_data_dir.argtypes = [C.c_char_p, C.c_char_p, C.c_uint64, C.c_double, C.c_int, C.c_uint64, C.c_uint64]
-    if lib.ref_write_data_dir(fasta.encode(), prefix.encode(), k, probability, seed, min_read_length, threads):
+    if ref_lib().ref_write_data_dir(fasta.encode(), prefix.encode(), k, probability, seed, min_read_length, threads):
         raise RuntimeError("reference failed to write the Data directory")
 
 
 def ref_open_vector(path, object_size):
     """(count, fnv checksum) of a MemoryMapped::Vector file as seen by the reference's own accessExistingReadOnly."""
-    lib = ref_lib()
-    lib.ref_open_vector.restype = C.c_int
-    lib.ref_open_vector.argtypes = [C.c_char_p, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_uint64)]
     n, h = C.c_uint64(), C.c_uint64()
-    rc = lib.ref_open_vector(path.encode(), object_size, C.byref(n), C.byref(h))
-    if rc:
+    if ref_lib().ref_open_vector(path.encode(), object_size, C.byref(n), C.byref(h)):
         raise RuntimeError(f"the reference could not open {path}")
     return n.value, h.value

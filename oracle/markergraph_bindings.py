@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE — ctypes bindings for createMarkerGraphVertices / findMarkerGraphReverseComplementVertices
 (src/AssemblerMarkerGraph.cpp): the C restatement in oracle/markergraph_oracle.c (part of oracle/_build/liboracle.so) and,
 when present, the reference's own DisjointSets, decompress and PeakFinder behind ref_glue/ref_markergraph.cpp in
-oracle/_ref/libshasta_ref_markergraph.so (built by oracle/markergraph.mk).
+oracle/_ref/libshasta_ref_markergraph.so (built by oracle/Makefile).
 
 Only tests/ and bench_markergraph.py may import this module. The product (shasta_b200/) never does.
 """
@@ -12,36 +12,44 @@ import os
 
 import numpy as np
 
-from oracle.bindings import oracle_lib
+from oracle import bindings
+from oracle._load import have, load, take
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-REF_MARKERGRAPH_SO = os.path.join(_HERE, "_ref", "libshasta_ref_markergraph.so")
-_ref = None
+REF_SO = os.path.join(_HERE, "_ref", "libshasta_ref_markergraph.so")
 
 DEFAULTS = dict(minCoverage=10, maxCoverage=100, minCoveragePerStrand=0, allowDuplicateMarkers=False,
                 peakFinderMinAreaFraction=0.08, peakFinderAreaStartIndex=2)
 
 
+_VERTICES = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
+             C.c_void_p, C.c_double] + [C.POINTER(C.c_void_p)] * 4 + [C.c_void_p]
+_RC = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
+_CUTOFF = [C.c_void_p, C.c_uint64, C.c_double, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_double)]
+_ORACLE_PROTOS = {
+    "orc_create_marker_graph_vertices": (C.c_int, _VERTICES),
+    "orc_find_rc_vertices": (C.c_int, _RC),
+    "orc_peak_finder_cutoff": (C.c_int, _CUTOFF),
+}
+_REF_PROTOS = {
+    "ref_create_marker_graph_vertices": (C.c_int, _VERTICES),
+    "ref_find_rc_vertices": (C.c_int, _RC),
+    "ref_peak_finder_cutoff": (C.c_int, _CUTOFF),
+    "ref_open_vector40": (C.c_int, [C.c_char_p, C.POINTER(C.c_uint64), C.POINTER(C.c_void_p)]),
+    "ref_free_markergraph": (None, [C.c_void_p]),
+}
+
+
+def oracle_lib():
+    return bindings.oracle_lib(_ORACLE_PROTOS)
+
+
 def have_ref():
-    return os.path.exists(REF_MARKERGRAPH_SO)
+    return have(REF_SO)
 
 
 def ref_lib():
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_MARKERGRAPH_SO)
-        _ref.ref_free_markergraph.argtypes = [C.c_void_p]
-    return _ref
-
-
-def _take(lib_free, p, n):
-    out = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint64)), (n,)).copy() if n else np.zeros(0, np.uint64)
-    lib_free(p)
-    return out
-
-
-_PROTO = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
-          C.c_double] + [C.POINTER(C.c_void_p)] * 4 + [C.c_void_p]
+    return load(REF_SO, _REF_PROTOS)
 
 
 def _run(f, lib_free, toc, kmer, edges, ctoc, cdata, flags, threads, **params):
@@ -58,16 +66,15 @@ def _run(f, lib_free, toc, kmer, edges, ctoc, cdata, flags, threads, **params):
                    d["peakFinderAreaStartIndex"], threads], np.uint64)
     counts = np.zeros(12, np.uint64)
     t, vt, vd, h = C.c_void_p(), C.c_void_p(), C.c_void_p(), C.c_void_p()
-    f.restype = C.c_int
-    f.argtypes = _PROTO
     status = f(toc.ctypes.data, R, kmer.ctypes.data, edges.ctypes.data, len(edges), ctoc.ctypes.data, cdata.ctypes.data,
                len(ctoc) - 1, flags.ctypes.data, pv.ctypes.data, float(d["peakFinderMinAreaFraction"]), C.byref(t), C.byref(vt),
                C.byref(vd), C.byref(h), counts.ctypes.data)
     if status:
         return dict(status=int(status))
     M, V = int(toc[-1]), int(counts[8])
-    return dict(status=0, table=_take(lib_free, t, M), vtoc=_take(lib_free, vt, V + 1), vdata=_take(lib_free, vd, int(counts[10])),
-                histogram=_take(lib_free, h, int(counts[9])), minCoverageUsed=int(counts[0]), peakFinderFailed=int(counts[1]),
+    return dict(status=0, table=take(t, M, np.uint64, lib_free), vtoc=take(vt, V + 1, np.uint64, lib_free),
+                vdata=take(vd, int(counts[10]), np.uint64, lib_free), histogram=take(h, int(counts[9]), np.uint64, lib_free),
+                minCoverageUsed=int(counts[0]), peakFinderFailed=int(counts[1]),
                 disjointSetCount=int(counts[5]), keptDisjointSetCount=int(counts[6]), badDisjointSetCount=int(counts[7]),
                 vertexCount=V, observedAreaFraction=float(counts[11:12].view(np.float64)[0]),
                 edgePairsUsed=int(counts[2]), edgePairsSkipped=int(counts[3]), alignedMarkerPairs=int(counts[4]))
@@ -93,8 +100,6 @@ def _rc(f, toc, table, vtoc, vdata):
     vdata = np.ascontiguousarray(vdata, np.uint64)
     V = len(vtoc) - 1
     rc = np.zeros(V + 1, np.uint64)
-    f.restype = C.c_int
-    f.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
     status = f(toc.ctypes.data, (len(toc) - 1) // 2, table.ctypes.data, vtoc.ctypes.data, vdata.ctypes.data, V, rc.ctypes.data)
     return int(status), rc[:V].copy()
 
@@ -110,20 +115,15 @@ def ref_find_rc_vertices(toc, table, vtoc, vdata):
 def ref_open_vector40(path):
     """(count, values uint64[count]) of a MemoryMapped::Vector<Uint40> file, opened by the reference's own code."""
     lib = ref_lib()
-    f = lib.ref_open_vector40
-    f.restype = C.c_int
-    f.argtypes = [C.c_char_p, C.POINTER(C.c_uint64), C.POINTER(C.c_void_p)]
     n, p = C.c_uint64(), C.c_void_p()
-    if f(path.encode(), C.byref(n), C.byref(p)):
+    if lib.ref_open_vector40(path.encode(), C.byref(n), C.byref(p)):
         raise RuntimeError(f"the reference could not open {path}")
-    return n.value, _take(lib.ref_free_markergraph, p, n.value)
+    return n.value, take(p, n.value, np.uint64, lib.ref_free_markergraph)
 
 
 def _cutoff(f, y, min_area_fraction, start_index):
     y = np.ascontiguousarray(y, np.uint64)
     cutoff, observed = C.c_uint64(0), C.c_double(0)
-    f.restype = C.c_int
-    f.argtypes = [C.c_void_p, C.c_uint64, C.c_double, C.c_uint64, C.POINTER(C.c_uint64), C.POINTER(C.c_double)]
     threw = f(y.ctypes.data, len(y), float(min_area_fraction), int(start_index), C.byref(cutoff), C.byref(observed))
     return int(threw), int(cutoff.value), float(observed.value)
 

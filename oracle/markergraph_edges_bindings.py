@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE — ctypes bindings for createMarkerGraphEdges / findMarkerGraphReverseComplementEdges
 (src/AssemblerMarkerGraph.cpp): the C restatement in oracle/markergraph_edges_oracle.c (part of oracle/_build/liboracle.so)
 and, when present, the reference's own MarkerGraph, MultithreadedObject and MemoryMapped containers behind
-ref_glue/ref_markergraph_edges.cpp in oracle/_ref/libshasta_ref_markergraph_edges.so (built by oracle/markergraph_edges.mk).
+ref_glue/ref_markergraph_edges.cpp in oracle/_ref/libshasta_ref_markergraph_edges.so (built by oracle/Makefile).
 
 Edge sets are dicts: edges uint8[E,14], intervalsToc uint64[E+1], intervalsData uint32[I,3], bySourceToc / byTargetToc
 uint64[V+1], bySourceData / byTargetData uint64[E]. Only tests/ and bench_markergraph_edges.py import this module.
@@ -13,38 +13,44 @@ import os
 
 import numpy as np
 
-from oracle.bindings import oracle_lib
+from oracle import bindings
+from oracle._load import have, load, take
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 REF_SO = os.path.join(_HERE, "_ref", "libshasta_ref_markergraph_edges.so")
-_ref = None
 INV40 = (1 << 40) - 1
+
+_EDGES = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
+_RC_EDGES = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64] + [C.c_void_p] * 4
+_ORACLE_PROTOS = {
+    "orc_create_marker_graph_edges": (C.c_int, _EDGES + [C.POINTER(C.c_void_p)] * 7 + [C.c_void_p]),
+    "orc_find_rc_edges": (C.c_int, _RC_EDGES + [C.c_void_p] * 2),
+}
+_REF_PROTOS = {
+    "ref_create_marker_graph_edges": (C.c_int, _EDGES + [C.c_uint64] + [C.POINTER(C.c_void_p)] * 7 + [C.c_void_p]),
+    "ref_find_rc_edges": (C.c_int, _RC_EDGES + [C.c_uint64, C.c_void_p, C.c_char_p, C.c_uint64]),
+    "ref_open_marker_graph_edges": (C.c_int, [C.c_char_p] * 5 + [C.POINTER(C.c_void_p)] * 8 + [C.c_void_p]),
+    "ref_free_markergraph_edges": (None, [C.c_void_p]),
+}
+
+
+def oracle_lib():
+    return bindings.oracle_lib(_ORACLE_PROTOS)
 
 
 def have_ref():
-    return os.path.exists(REF_SO)
+    return have(REF_SO)
 
 
 def ref_lib():
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_SO)
-        _ref.ref_free_markergraph_edges.argtypes = [C.c_void_p]
-    return _ref
-
-
-def _take(free, p, n, dtype):
-    dtype = np.dtype(dtype)
-    out = np.ctypeslib.as_array(C.cast(p, C.POINTER(C.c_uint8)), (n * dtype.itemsize,)).view(dtype).copy() if n else np.zeros(0, dtype)
-    free(p)
-    return out
+    return load(REF_SO, _REF_PROTOS)
 
 
 def _edge_set(free, ptrs, E, I, V):
-    return dict(edges=_take(free, ptrs[0], 14 * E, np.uint8).reshape(-1, 14), intervalsToc=_take(free, ptrs[1], E + 1, np.uint64),
-                intervalsData=_take(free, ptrs[2], 3 * I, np.uint32).reshape(-1, 3), bySourceToc=_take(free, ptrs[3], V + 1, np.uint64),
-                bySourceData=_take(free, ptrs[4], E, np.uint64), byTargetToc=_take(free, ptrs[5], V + 1, np.uint64),
-                byTargetData=_take(free, ptrs[6], E, np.uint64))
+    return dict(edges=take(ptrs[0], 14 * E, np.uint8, free).reshape(-1, 14), intervalsToc=take(ptrs[1], E + 1, np.uint64, free),
+                intervalsData=take(ptrs[2], 3 * I, np.uint32, free).reshape(-1, 3), bySourceToc=take(ptrs[3], V + 1, np.uint64, free),
+                bySourceData=take(ptrs[4], E, np.uint64, free), byTargetToc=take(ptrs[5], V + 1, np.uint64, free),
+                byTargetData=take(ptrs[6], E, np.uint64, free))
 
 
 def _u64(a):
@@ -54,15 +60,12 @@ def _u64(a):
 def oracle_create_marker_graph_edges(toc, table, vtoc, vdata):
     """The C restatement (one thread's output). table, vtoc: uint64. Returns dict(status, the edge set, saturated)."""
     lib = oracle_lib()
-    f = lib.orc_create_marker_graph_edges
-    f.restype = C.c_int
-    f.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64] + [C.POINTER(C.c_void_p)] * 7 + [C.c_void_p]
     toc, table, vtoc, vdata = _u64(toc), _u64(table), _u64(vtoc), _u64(vdata)
     V = len(vtoc) - 1
     ptrs = [C.c_void_p() for _ in range(7)]
     counts = np.zeros(3, np.uint64)
-    status = f(toc.ctypes.data, (len(toc) - 1) // 2, table.ctypes.data, vtoc.ctypes.data, vdata.ctypes.data, V,
-               *[C.byref(p) for p in ptrs], counts.ctypes.data)
+    status = lib.orc_create_marker_graph_edges(toc.ctypes.data, (len(toc) - 1) // 2, table.ctypes.data, vtoc.ctypes.data,
+                                               vdata.ctypes.data, V, *[C.byref(p) for p in ptrs], counts.ctypes.data)
     if status:
         return dict(status=int(status))
     out = _edge_set(lib.orc_free, ptrs, int(counts[0]), int(counts[1]), V)
@@ -73,16 +76,12 @@ def oracle_create_marker_graph_edges(toc, table, vtoc, vdata):
 def ref_create_marker_graph_edges(toc, table, vtoc, vdata, threads=1):
     """The reference's objects in the members' control flow. threads=0: all cores."""
     lib = ref_lib()
-    f = lib.ref_create_marker_graph_edges
-    f.restype = C.c_int
-    f.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64] + [C.POINTER(C.c_void_p)] * 7 + \
-        [C.c_void_p]
     toc, table, vtoc, vdata = _u64(toc), _u64(table), _u64(vtoc), _u64(vdata)
     V = len(vtoc) - 1
     ptrs = [C.c_void_p() for _ in range(7)]
     counts = np.zeros(2, np.uint64)
-    status = f(toc.ctypes.data, (len(toc) - 1) // 2, table.ctypes.data, vtoc.ctypes.data, vdata.ctypes.data, V, threads,
-               *[C.byref(p) for p in ptrs], counts.ctypes.data)
+    status = lib.ref_create_marker_graph_edges(toc.ctypes.data, (len(toc) - 1) // 2, table.ctypes.data, vtoc.ctypes.data,
+                                               vdata.ctypes.data, V, threads, *[C.byref(p) for p in ptrs], counts.ctypes.data)
     if status:
         return dict(status=int(status))
     out = _edge_set(lib.ref_free_markergraph_edges, ptrs, int(counts[0]), int(counts[1]), V)
@@ -99,8 +98,6 @@ def oracle_find_rc_edges(toc, rc_vertex, s):
     """(message or None, rc uint64[E]) of the C restatement on edge set s. The messages are the reference's (the assertion's
     without its location)."""
     f = oracle_lib().orc_find_rc_edges
-    f.restype = C.c_int
-    f.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64] + [C.c_void_p, C.c_uint64] + [C.c_void_p] * 6
     toc, rv = _u64(toc), _u64(rc_vertex)
     e = np.ascontiguousarray(s["edges"], np.uint8)
     E = len(e)
@@ -117,9 +114,6 @@ def oracle_find_rc_edges(toc, rc_vertex, s):
 def ref_find_rc_edges(toc, rc_vertex, s, threads=1):
     """(message or None, rc uint64[E]) of the reference's member on edge set s."""
     f = ref_lib().ref_find_rc_edges
-    f.restype = C.c_int
-    f.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64] + [C.c_void_p] * 4 + \
-        [C.c_uint64, C.c_void_p, C.c_char_p, C.c_uint64]
     toc, rv = _u64(toc), _u64(rc_vertex)
     e = np.ascontiguousarray(s["edges"], np.uint8)
     E = len(e)
@@ -136,21 +130,18 @@ def ref_find_rc_edges(toc, rc_vertex, s, threads=1):
 def ref_open_marker_graph_edges(prefix, with_rc=True):
     """The five file sets the facade writes under prefix (Data/), opened by the reference's own MemoryMapped code."""
     lib = ref_lib()
-    f = lib.ref_open_marker_graph_edges
-    f.restype = C.c_int
-    f.argtypes = [C.c_char_p] * 5 + [C.POINTER(C.c_void_p)] * 8 + [C.c_void_p]
     ptrs = [C.c_void_p() for _ in range(8)]
     counts = np.zeros(4, np.uint64)
     names = [prefix + n for n in ("GlobalMarkerGraphEdges", "GlobalMarkerGraphEdgeMarkerIntervals", "GlobalMarkerGraphEdgesBySource",
                                   "GlobalMarkerGraphEdgesByTarget")]
     rc_path = (prefix + "MarkerGraphReverseComplementeEdge").encode() if with_rc else None
-    if f(*[n.encode() for n in names], rc_path, *[C.byref(p) for p in ptrs], counts.ctypes.data):
+    if lib.ref_open_marker_graph_edges(*[n.encode() for n in names], rc_path, *[C.byref(p) for p in ptrs], counts.ctypes.data):
         raise RuntimeError(f"the reference could not open the marker graph edges under {prefix}")
     E, I, V = int(counts[0]), int(counts[1]), int(counts[2])
     assert int(counts[3]) == V
     out = _edge_set(lib.ref_free_markergraph_edges, ptrs[:7], E, I, V)
     if with_rc:
-        out["rc"] = _take(lib.ref_free_markergraph_edges, ptrs[7], E, np.uint64)
+        out["rc"] = take(ptrs[7], E, np.uint64, lib.ref_free_markergraph_edges)
     return out
 
 

@@ -1,7 +1,7 @@
 """TEST INFRASTRUCTURE — flagCrossStrandReadGraphEdges1 and flagChimericReads (src/AssemblerReadGraph.cpp:355-583, 775-1041):
 a plain restatement in Python (breadth-first searches over the read graph, the regions processed with a STABLE sort) and,
 when present, the reference's own ReadGraph behind ref_glue/ref_readgraph_flags.cpp in
-oracle/_ref/libshasta_ref_readgraph_flags.so (built by oracle/readgraph_flags.mk).
+oracle/_ref/libshasta_ref_readgraph_flags.so (built by oracle/Makefile).
 
 The restatement of the region step equals the reference whenever no two edge pairs of a region tie on markerCount (the
 reference's two std::sort calls are unstable); region_ties() says whether an input has such a tie. Everything else is a
@@ -17,27 +17,27 @@ from collections import deque
 
 import numpy as np
 
+from oracle._load import have, load
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 REF_SO = os.path.join(_HERE, "_ref", "libshasta_ref_readgraph_flags.so")
-_ref = None
 CROSS = np.uint32(1 << 30)          # crossesStrands: bit 62 of the second 64-bit word = bit 30 of word 3
+
+_REF_PROTOS = {
+    "ref_flag_cross_strand_read_graph_edges1": (C.c_int, [C.c_int64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64,
+                                                          C.c_void_p, C.c_uint64, C.c_void_p]),
+    "ref_flag_chimeric_reads": (C.c_int, [C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
+                                          C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p]),
+    "ref_open_read_graph_edges": (C.c_int, [C.c_char_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]),
+}
 
 
 def have_ref():
-    return os.path.exists(REF_SO)
+    return have(REF_SO)
 
 
 def ref_lib():
-    global _ref
-    if _ref is None:
-        _ref = C.CDLL(REF_SO)
-        _ref.ref_flag_cross_strand_read_graph_edges1.restype = C.c_int
-        _ref.ref_flag_cross_strand_read_graph_edges1.argtypes = [C.c_int64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64,
-                                                                  C.c_void_p, C.c_uint64, C.c_void_p]
-        _ref.ref_flag_chimeric_reads.restype = C.c_int
-        _ref.ref_flag_chimeric_reads.argtypes = [C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p,
-                                                 C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p]
-    return _ref
+    return load(REF_SO, _REF_PROTOS)
 
 
 def _inputs(g):
@@ -71,12 +71,9 @@ def ref_chimeric(g, max_distance, threads=1):
 
 def ref_open_read_graph_edges(path, capacity):
     """uint32[n, 4] of a Data/ReadGraphEdges file, opened by the reference's MemoryMapped::Vector<ReadGraphEdge>."""
-    f = ref_lib().ref_open_read_graph_edges
-    f.restype = C.c_int
-    f.argtypes = [C.c_char_p, C.c_void_p, C.c_uint64, C.POINTER(C.c_uint64)]
     out = np.zeros((capacity, 4), np.uint32)
     n = C.c_uint64()
-    if f(path.encode(), out.ctypes.data, capacity, C.byref(n)):
+    if ref_lib().ref_open_read_graph_edges(path.encode(), out.ctypes.data, capacity, C.byref(n)):
         raise RuntimeError(f"the reference could not open {path}")
     return out[:min(n.value, capacity)], n.value
 

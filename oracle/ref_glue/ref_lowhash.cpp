@@ -5,7 +5,7 @@
 // and bench.py --impl reference can run the real reference code.
 //
 // This TU is compiled together with reference translation units taken from
-// /root/reference/src where they lie (see oracle/Makefile, target _ref); no
+// /root/reference/src where they lie (see oracle/Makefile, target ref); no
 // reference source is copied into this repository. Output: oracle/_ref/libshasta_ref.so
 //
 // Reference entry points driven from here:

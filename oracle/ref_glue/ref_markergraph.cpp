@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE — NOT PRODUCT CODE.
 // extern "C" access to Assembler::createMarkerGraphVertices (src/AssemblerMarkerGraph.cpp:38-518, threads :522-770) and
-// findMarkerGraphReverseComplementVertices (:1134-1230), built by oracle/markergraph.mk into
+// findMarkerGraphReverseComplementVertices (:1134-1230), built by oracle/Makefile into
 // oracle/_ref/libshasta_ref_markergraph.so. Assembler cannot be linked here, so this glue follows the members' control flow
 // over the reference's own components, compiled unmodified from where they lie:
 //   DisjointSets          src/dset64-gccAtomic.hpp   (concurrent union-find, used by threadCount threads as in :124-152)

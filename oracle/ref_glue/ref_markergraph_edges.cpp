@@ -1,7 +1,7 @@
 // TEST INFRASTRUCTURE — NOT PRODUCT CODE.
 // extern "C" access to Assembler::createMarkerGraphEdges (src/AssemblerMarkerGraph.cpp:2028-2085, worker :2116-2180,
 // children :1025-1080), createMarkerGraphEdgesBySourceAndTarget (:2089-2112, :2192-2213) and
-// findMarkerGraphReverseComplementEdges (:1244-1389), built by oracle/markergraph_edges.mk into
+// findMarkerGraphReverseComplementEdges (:1244-1389), built by oracle/Makefile into
 // oracle/_ref/libshasta_ref_markergraph_edges.so. Assembler cannot be linked here, so this glue follows the members' control
 // flow over the reference's own objects, compiled unmodified from where they lie:
 //   shasta::MarkerGraph           src/MarkerGraph.cpp (its Edge, vertices, vertexTable, edges, edgeMarkerIntervals,

@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE — NOT PRODUCT CODE.
 // extern "C" access to the reference's palindromic-read decision, compiled unmodified from the reference tree by
-// oracle/palindromic.mk into oracle/_ref/libshasta_ref_palindromic.so:
+// oracle/Makefile into oracle/_ref/libshasta_ref_palindromic.so:
 //   getMarkersSortedByKmerId        src/AssemblerMarkers.cpp:83-98   (restated here: std::sort of MarkerWithOrdinal)
 //   shasta::align / AlignmentGraph  src/AlignmentGraph.cpp:14-136    (compiled unmodified, with ref_glue/shims/boost/graph)
 //   the two thresholds              src/AssemblerAlign.cpp:741-766   (restated here)

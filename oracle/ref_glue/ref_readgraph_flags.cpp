@@ -1,6 +1,6 @@
 // TEST INFRASTRUCTURE — NOT PRODUCT CODE.
 // extern "C" access to Assembler::flagCrossStrandReadGraphEdges1 (src/AssemblerReadGraph.cpp:775-1041) and
-// Assembler::flagChimericReads (:355-583), built by oracle/readgraph_flags.mk into oracle/_ref/libshasta_ref_readgraph_flags.so.
+// Assembler::flagChimericReads (:355-583), built by oracle/Makefile into oracle/_ref/libshasta_ref_readgraph_flags.so.
 // Assembler cannot be linked here, so this glue follows the members' control flow over the reference's own objects,
 // compiled unmodified from where they lie:
 //   ReadGraph, ReadGraphEdge, ReadGraph::computeShortPath   src/ReadGraph.{hpp,cpp}

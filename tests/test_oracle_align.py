@@ -34,7 +34,7 @@ def test_compress_worked_example():
 
 
 def test_reference_selftest_and_compress_vectors():
-    assert recorded("align", "selftest", lambda: B._rlib().ref_test_alignment_compression()) == 0
+    assert recorded("align", "selftest", lambda: B.ref_lib().ref_test_alignment_compression()) == 0
     rng = np.random.default_rng(1)
     for trial in range(200):
         n = int(rng.integers(1, 60))
