@@ -142,17 +142,6 @@ def lib():
                                          C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
         L.shb_device_free.argtypes = [C.c_void_p]
         L.shb_markers_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
-        L.shb_lowhash_begin.argtypes = [C.c_void_p, C.POINTER(LowHashParams), C.POINTER(C.c_uint64)]
-        L.shb_lowhash_sweep.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p]
-        L.shb_lowhash_slab.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-        L.shb_device_partition.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_void_p,
-                                           C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
-        L.shb_lowhash_process_entries.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
-        L.shb_lowhash_local_pairs.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
-        L.shb_lowhash_set_pairs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
-        L.shb_lowhash_emit.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_uint64)]
-        L.shb_lowhash_stats_device.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-        L.shb_lowhash_counters.argtypes = [C.c_void_p, C.POINTER(LowHashResult)]
         L.shb_copy_device_to_host.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
         L.shb_test_radix_sort.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_int]
         L.shb_create_read_graph2.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64, C.c_uint32, C.c_double, C.c_double,

@@ -23,15 +23,6 @@ void computeAlignments(shb_context* c, const void* candidatesHost, uint64_t n, c
 void destroyAlignCache(shb_context* c);
 void destroyLowhashState(shb_context* c);
 void destroyDistState(shb_context* c);
-LowHashState& lowhashState(shb_context* c);
-void lowhashBegin(shb_context* c, const shb_lowhash_params& p);
-void lowhashSweep(shb_context* c, uint64_t iterationBegin, uint32_t group, unsigned long long* counts);
-void lowhashProcessEntries(shb_context* c, uint64_t* keysA, uint32_t* valsA, uint64_t n64);
-void lowhashLocalPairs(shb_context* c, uint64_t** keys, uint32_t** counts, uint64_t* n);
-void lowhashSetPairs(shb_context* c, const uint64_t* keys, const uint32_t* counts, uint64_t n);
-void lowhashEmit(shb_context* c, void** candidatesOut, uint64_t* candidateCountOut);
-void devicePartition(shb_context* c, uint64_t* keys, uint32_t* vals, uint64_t n, uint32_t shift, uint32_t bits,
-                     uint64_t* counts, uint64_t** keysOut, uint32_t** valsOut);
 void computeAlignmentTable(shb_context* c, const void* alignmentData, uint64_t n, uint64_t readCount, uint32_t** tocOut, uint32_t** dataOut);
 void findMarkers(shb_context* c, uint32_t k, uint64_t readCount, const uint64_t* wordOffsets, const uint64_t* words,
                  const uint64_t* baseCounts, const uint8_t* kmerTable24, const uint32_t* isMarkerBitmap,
@@ -231,105 +222,6 @@ shb_status shb_markers_device(shb_context* c, void** kmerIdsDevice, uint64_t* lo
         SHB_REQUIRE(c->haveMarkers, SHB_ERR_STATE, "Markers are not accessible.");
         *kmerIdsDevice = const_cast<uint32_t*>(c->kmerIds);
         *localMarkerCount = c->localMarkerCount;
-    });
-}
-
-shb_status shb_lowhash_begin(shb_context* c, const shb_lowhash_params* params, uint64_t* log2BucketCount)
-{
-    return guarded([&] {
-        SHB_REQUIRE(c && params, SHB_ERR_INVALID, "Null argument.");
-        lowhashBegin(c, *params);
-        if(log2BucketCount) *log2BucketCount = lowhashState(c).log2BucketCount;
-    });
-}
-
-shb_status shb_lowhash_sweep(shb_context* c, uint64_t iterationBegin, uint32_t iterationCount, uint64_t* lowHashCounts)
-{
-    return guarded([&] {
-        SHB_REQUIRE(c && lowHashCounts, SHB_ERR_INVALID, "Null argument.");
-        unsigned long long counts[64] = {0};
-        SHB_REQUIRE(iterationCount <= 64, SHB_ERR_INVALID, "Invalid iteration group.");
-        lowhashSweep(c, iterationBegin, iterationCount, counts);
-        for(uint32_t s = 0; s < iterationCount; s++) lowHashCounts[s] = counts[s];
-    });
-}
-
-shb_status shb_lowhash_slab(shb_context* c, uint32_t slab, void** keysDevice, void** valsDevice)
-{
-    return guarded([&] {
-        SHB_REQUIRE(c && keysDevice && valsDevice, SHB_ERR_INVALID, "Null argument.");
-        LowHashState& S = lowhashState(c);
-        SHB_REQUIRE(S.active && slab < S.slabGroup, SHB_ERR_STATE, "No such slab.");
-        *keysDevice = c->sweepKeys.get() + uint64_t(slab) * S.capacity;
-        *valsDevice = c->sweepVals.get() + uint64_t(slab) * S.capacity;
-    });
-}
-
-shb_status shb_device_partition(shb_context* c, void* keysDevice, void* valsDevice, uint64_t n, uint32_t shift, uint32_t bits,
-                                uint64_t* counts, void** keysOutDevice, void** valsOutDevice)
-{
-    return guarded([&] {
-        SHB_REQUIRE(c && counts && keysOutDevice && valsOutDevice && ((keysDevice && valsDevice) || n == 0), SHB_ERR_INVALID, "Null argument.");
-        uint64_t* ko = nullptr; uint32_t* vo = nullptr;
-        devicePartition(c, static_cast<uint64_t*>(keysDevice), static_cast<uint32_t*>(valsDevice), n, shift, bits, counts, &ko, &vo);
-        *keysOutDevice = ko; *valsOutDevice = vo;
-    });
-}
-
-shb_status shb_lowhash_process_entries(shb_context* c, void* keysDevice, void* valsDevice, uint64_t n)
-{
-    return guarded([&] {
-        SHB_REQUIRE(c && ((keysDevice && valsDevice) || n == 0), SHB_ERR_INVALID, "Null argument.");
-        lowhashProcessEntries(c, static_cast<uint64_t*>(keysDevice), static_cast<uint32_t*>(valsDevice), n);
-        SHB_CUDA(cudaStreamSynchronize(c->stream));
-    });
-}
-
-shb_status shb_lowhash_local_pairs(shb_context* c, void** pairKeysDevice, void** pairCountsDevice, uint64_t* n)
-{
-    return guarded([&] {
-        SHB_REQUIRE(c && pairKeysDevice && pairCountsDevice && n, SHB_ERR_INVALID, "Null argument.");
-        uint64_t* k = nullptr; uint32_t* v = nullptr;
-        lowhashLocalPairs(c, &k, &v, n);
-        SHB_CUDA(cudaStreamSynchronize(c->stream));
-        *pairKeysDevice = k; *pairCountsDevice = v;
-    });
-}
-
-shb_status shb_lowhash_set_pairs(shb_context* c, const void* pairKeysDevice, const void* pairCountsDevice, uint64_t n)
-{
-    return guarded([&] {
-        SHB_REQUIRE(c && ((pairKeysDevice && pairCountsDevice) || n == 0), SHB_ERR_INVALID, "Null argument.");
-        lowhashSetPairs(c, static_cast<const uint64_t*>(pairKeysDevice), static_cast<const uint32_t*>(pairCountsDevice), n);
-    });
-}
-
-shb_status shb_lowhash_emit(shb_context* c, void** candidates, uint64_t* candidateCount)
-{
-    return guarded([&] {
-        SHB_REQUIRE(c && candidates && candidateCount, SHB_ERR_INVALID, "Null argument.");
-        lowhashEmit(c, candidates, candidateCount);
-    });
-}
-
-shb_status shb_lowhash_stats_device(shb_context* c, void** statsDevice)
-{
-    return guarded([&] {
-        SHB_REQUIRE(c && statsDevice, SHB_ERR_INVALID, "Null argument.");
-        SHB_REQUIRE(lowhashState(c).active, SHB_ERR_STATE, "shb_lowhash_begin was not called.");
-        *statsDevice = c->stats.get();
-    });
-}
-
-shb_status shb_lowhash_counters(shb_context* c, shb_lowhash_result* result)
-{
-    return guarded([&] {
-        SHB_REQUIRE(c && result, SHB_ERR_INVALID, "Null argument.");
-        LowHashState& S = lowhashState(c);
-        memset(result, 0, sizeof(*result));
-        result->log2BucketCount = S.log2BucketCount; result->lowHashCount = S.lowHashCount; result->pairCount = S.pairCount;
-        result->sweepMs = S.sweepMs; result->sweepLaunches = S.sweepLaunches; result->kernelLaunches = g_launchCount;
-        result->candidateCount = S.emittedCount; result->candidateDigest = S.candidateDigest;
     });
 }
 

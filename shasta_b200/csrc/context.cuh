@@ -65,17 +65,17 @@ struct LowHashAccumulator {
     uint64_t rawCount = 0;  // raw pair hits (one key per hit, any order) of the iterations since the last reduction, in pairsA
     uint64_t rawLimit = 1ull << 31;     // reduce the raw hits when one more iteration would exceed this many (SHB_LOWHASH_RAW_LIMIT)
 };
-// State of a staged LowHash0 run (shb_lowhash_begin ... shb_lowhash_emit).
+// State of one LowHash0 run (lowhashBegin ... lowhashEmitDevice in lowhash.cu), on one GPU (lowhash0) or on one rank of a
+// read-sharded run (dist.cu).
 struct LowHashState {
-    bool active = false;
     shb_lowhash_params p{};
     uint64_t log2BucketCount = 0, bucketMask = 0, hashThreshold = 0, capacity = 0;
-    uint32_t readBits = 1, slabGroup = 0;
+    uint32_t readBits = 1;
     uint32_t queueCapacityOverride = 0; // SHB_LOWHASH_QUEUE_CAPACITY (test hook), 0 = derived from hashFraction
     bool aggregateByRead = false;       // pair hits are counted per read in shared memory before they reach the accumulator
     LowHashAccumulator acc;
     uint64_t lowHashCount = 0, pairCount = 0, sweepLaunches = 0;
-    uint64_t emittedCount = 0, candidateDigest = 0;     // of the last shb_lowhash_emit
+    uint64_t emittedCount = 0, candidateDigest = 0;     // of the last lowhashEmitDevice
     double sweepMs = 0.;
 };
 }

@@ -15,8 +15,8 @@
 //   * ReadLowHashStatistics are partial sums, all-reduced once;
 //   * alignment: the k-mer id shards are gathered once per marker set (grouped ncclBroadcast, cached until the markers
 //     change) into a second context that then aligns this rank's block of candidates; no collective in the loop.
-// The Python twin of the routing logic (shasta_b200/distributed.py over torch.distributed) is what the CPU tests cover
-// with gloo; this file is what bench.py and a C++ host run on GPUs.
+// bench.py --gpus N, tests/run_distributed_gpu.py and a C++ host run this file on GPUs; tests/test_gpu_distributed.py runs it
+// as a world of one.
 #include "context.cuh"
 #include "hostpool.cuh"
 

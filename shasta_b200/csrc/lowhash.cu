@@ -178,9 +178,9 @@ uint32_t nextSweepGroup(uint64_t remaining, uint64_t slabCapacity) { return next
 
 
 // ---------------------------------------------------------------------------------------------
-// Staged LowHash0. The single-GPU call is begin -> { sweep -> processEntries per slab } -> finish;
-// a multi-GPU run inserts the bucket exchange between sweep and processEntries and the pair exchange
-// before emit (shasta_b200/distributed.py).
+// LowHash0 in stages. The single-GPU call (lowhash0) is begin -> { sweep -> processEntries per slab } -> emit; the
+// read-sharded run (dist.cu) inserts the bucket exchange between sweep and processEntries and the pair exchange
+// (localPairs -> setPairs) before emit.
 LowHashState& lowhashState(shb_context* c)
 {
     if(!c->lowhashState) c->lowhashState = new LowHashState();
@@ -237,7 +237,6 @@ void lowhashBegin(shb_context* c, const shb_lowhash_params& p)
     if(S.capacity > M + 1) S.capacity = M + 1;
     c->stats.reserve(3 * R + 1);
     SHB_CUDA(cudaMemsetAsync(c->stats.get(), 0, (3 * R + 1) * sizeof(unsigned long long), st));
-    S.active = true;
 }
 
 // pass 1 for `group` consecutive iterations in one pass over the local k-mer ids. counts[s] = low hashes of
@@ -245,7 +244,6 @@ void lowhashBegin(shb_context* c, const shb_lowhash_params& p)
 void lowhashSweep(shb_context* c, uint64_t iterationBegin, uint32_t group, unsigned long long* counts)
 {
     LowHashState& S = lowhashState(c);
-    SHB_REQUIRE(S.active, SHB_ERR_STATE, "shb_lowhash_begin was not called.");
     SHB_REQUIRE(group >= 1 && group <= (uint32_t)kMaxFusedIterations, SHB_ERR_INVALID, "Invalid iteration group.");
     SHB_CUDA(cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
@@ -299,7 +297,6 @@ void lowhashSweep(shb_context* c, uint64_t iterationBegin, uint32_t group, unsig
         if(worst <= S.capacity) break;
         S.capacity = worst + worst / 8 + 1024;        // slab overflow: grow and redo this group
     }
-    S.slabGroup = group;
 }
 
 // passes 2 and 3 on one iteration's entries (keys = bucketId<<32 | hashHigh, vals = orientedReadId), which must all
@@ -309,7 +306,6 @@ void lowhashSweep(shb_context* c, uint64_t iterationBegin, uint32_t group, unsig
 void lowhashProcessEntries(shb_context* c, uint64_t* keysA, uint32_t* valsA, uint64_t n64)
 {
     LowHashState& S = lowhashState(c);
-    SHB_REQUIRE(S.active, SHB_ERR_STATE, "shb_lowhash_begin was not called.");
     SHB_REQUIRE(n64 < (1ull << 32), SHB_ERR_INVALID, "LowHash0: more than 2^32-1 low hashes in one iteration.");
     SHB_CUDA(cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
@@ -402,7 +398,6 @@ void lowhashProcessEntries(shb_context* c, uint64_t* keysA, uint32_t* valsA, uin
 void lowhashLocalPairs(shb_context* c, uint64_t** keys, uint32_t** counts, uint64_t* n)
 {
     LowHashState& S = lowhashState(c);
-    SHB_REQUIRE(S.active, SHB_ERR_STATE, "shb_lowhash_begin was not called.");
     SHB_CUDA(cudaSetDevice(c->device));
     reduceRawPairs(c, S.acc, S.readBits);
     mergeAccumulator(c, S.acc, S.readBits);
@@ -413,7 +408,6 @@ void lowhashLocalPairs(shb_context* c, uint64_t** keys, uint32_t** counts, uint6
 void lowhashSetPairs(shb_context* c, const uint64_t* keys, const uint32_t* counts, uint64_t n)
 {
     LowHashState& S = lowhashState(c);
-    SHB_REQUIRE(S.active, SHB_ERR_STATE, "shb_lowhash_begin was not called.");
     SHB_CUDA(cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     const uint64_t rawLimit = S.acc.rawLimit;
@@ -433,7 +427,6 @@ void lowhashSetPairs(shb_context* c, const uint64_t* keys, const uint32_t* count
 uint64_t lowhashEmitDevice(shb_context* c)
 {
     LowHashState& S = lowhashState(c);
-    SHB_REQUIRE(S.active, SHB_ERR_STATE, "shb_lowhash_begin was not called.");
     SHB_CUDA(cudaSetDevice(c->device));
     cudaStream_t st = c->stream;
     reduceRawPairs(c, S.acc, S.readBits);
@@ -536,7 +529,7 @@ void lowhash0(shb_context* c, const shb_lowhash_params& p,
 {
     SHB_REQUIRE(c->haveMarkers, SHB_ERR_STATE, "Markers are not accessible.");
     SHB_REQUIRE(c->readBegin == 0 && c->readEnd == c->readCountTotal, SHB_ERR_STATE,
-                "shb_lowhash0 needs all reads on this GPU (use the staged multi-GPU calls otherwise).");
+                "shb_lowhash0 needs all reads on this GPU (use shb_lowhash0_sharded otherwise).");
     const uint64_t R = c->readCountTotal;
     if(R == 0) {        // the reference would spin forever on 0/0 in its iteration control; return nothing
         *candidatesOut = malloc(1);

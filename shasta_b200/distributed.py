@@ -1,39 +1,7 @@
-"""Read-sharded multi-GPU LowHash0 + alignment (one process per GPU, torch.distributed for the plumbing).
-
-Sharding (SURVEY.md section 8e, BASELINE.json configs[2]):
-  * rank g holds the marker rows of a contiguous read range [readBegin_g, readEnd_g) and hashes only those;
-  * LowHash buckets are owned by ranks: owner(bucketId) = bucketId >> (log2BucketCount - log2 W). After every sweep the
-    low-hash entries of each iteration are grouped by owner on the device (one radix pass) and exchanged with ONE
-    all-to-all-v per iteration (NCCL over NVLink on GPUs; gloo in the CPU tests) — a bucket is never split across
-    ranks, so bucket sizes, per-read statistics and pair hits are exact;
-  * each owner accumulates (pair,count) for its buckets over all iterations; once, at the end, the merged local
-    lists are grouped by owner(readId0) = readId0 >> (readBits - log2 W) and exchanged; the owner sums, applies the
-    uint16 wrap and the minFrequency threshold, and emits its slice. Concatenating the slices in rank order gives
-    the reference's output order exactly;
-  * ReadLowHashStatistics are partial sums, all-reduced once;
-  * alignment: the k-mer ids are all-gathered so that every GPU holds all rows, and each rank aligns the candidates
-    it emitted (no collective in the loop).
-
-The orchestration below is written against a small `stages` interface so that its routing logic is covered on CPU
-(world_size 2, gloo) with a numpy stand-in (tests/test_distributed_cpu.py); on GPUs `CudaStages` drives the C ABI.
-"""
+"""Read ranges of equal marker weight for the ranks of a read-sharded run (the sharded path itself is csrc/dist.cu)."""
 from __future__ import annotations
 
 import numpy as np
-import torch
-import torch.distributed as dist
-
-
-def _log2_exact(n):
-    b = n.bit_length() - 1
-    if n < 1 or (1 << b) != n:
-        raise ValueError("the number of ranks must be a power of two")
-    return b
-
-
-def read_bits(read_count):
-    """Bits needed for readCount-1 (at least 1) — same rule as the library (lowhash.cu bitsFor)."""
-    return max(1, int(read_count - 1).bit_length()) if read_count else 1
 
 
 def balanced_read_ranges(weights, world):
@@ -48,274 +16,3 @@ def balanced_read_ranges(weights, world):
     for g in range(1, world + 1):
         bounds[g] = max(bounds[g], bounds[g - 1])
     return bounds
-
-
-def all_to_all_v(send, send_counts, group=None):
-    """Variable-size all-to-all of a 1-D tensor grouped by destination. Returns (recv, recv_counts)."""
-    world = dist.get_world_size(group)
-    sc = torch.tensor(send_counts, dtype=torch.int64, device=send.device)
-    rc = torch.empty(world, dtype=torch.int64, device=send.device)
-    dist.all_to_all_single(rc, sc, group=group)
-    recv_counts = [int(x) for x in rc.tolist()]
-    recv = torch.empty(sum(recv_counts), dtype=send.dtype, device=send.device)
-    dist.all_to_all_single(recv, send, recv_counts, [int(x) for x in send_counts], group=group)
-    return recv, recv_counts
-
-
-def lowhash0_sharded(stages, params, read_count_total, group=None):
-    """LowHash0 over read shards. `stages` implements the per-rank device stages (see CudaStages).
-    params: dict with the reference's argument names. Returns (local candidates uint32[n,3], stats tensor int64[R*3]
-    all-reduced, info dict). Every rank returns the slice of candidates whose readId0 it owns."""
-    world = dist.get_world_size(group)
-    log2w = _log2_exact(world)
-    iterations = int(params["minHashIterationCount"])
-    if iterations == 0:
-        raise ValueError("the sharded path needs a fixed minHashIterationCount (all shipped configurations use one); "
-                         "the candidate-driven stopping rule needs a merge per iteration")
-    import time
-    timing = {"sweep": 0.0, "partition": 0.0, "exchange": 0.0, "process": 0.0, "final": 0.0}
-
-    def tick():
-        if torch.cuda.is_available():
-            torch.cuda.synchronize()
-        return time.perf_counter()
-
-    log2_buckets = stages.begin(params)
-    if log2_buckets < log2w:
-        raise ValueError("fewer buckets than ranks")
-    entry_shift = 32 + log2_buckets - log2w
-    exchanged = 0
-    it = 0
-    while it < iterations:
-        group_size = min(stages.max_fused_iterations, iterations - it)
-        t0 = tick()
-        counts = stages.sweep(it, group_size)
-        t1 = tick()
-        timing["sweep"] += t1 - t0
-        # Group every slab by bucket owner first (device scratch is reused by each call), keep torch copies.
-        staged = []
-        for s in range(group_size):
-            keys, vals = stages.slab(s, counts[s])
-            pk, pv, pc = stages.partition(keys, vals, entry_shift, log2w)
-            staged.append((pk.clone(), pv.clone(), pc))
-        t2 = tick()
-        timing["partition"] += t2 - t1
-        # One exchange for the whole iteration group: slab after slab in each destination's segment would need a
-        # second sort at the receiver, so the slabs are exchanged one by one but the count exchange is batched.
-        send_counts = torch.tensor([pc for _, _, pc in staged], dtype=torch.int64, device=staged[0][0].device)    # [group, world]
-        received = []
-        rc_all = _exchange_counts(send_counts, group)
-        for s, (pk, pv, pc) in enumerate(staged):
-            rc = [int(x) for x in rc_all[s].tolist()]
-            rk = torch.empty(sum(rc), dtype=pk.dtype, device=pk.device)
-            rv = torch.empty(sum(rc), dtype=pv.dtype, device=pv.device)
-            dist.all_to_all_single(rk, pk, rc, pc, group=group)
-            dist.all_to_all_single(rv, pv, rc, pc, group=group)
-            received.append((rk, rv))
-        t3 = tick()
-        timing["exchange"] += t3 - t2
-        for rk, rv in received:
-            exchanged += int(rk.numel())
-            stages.process_entries(rk, rv)
-        timing["process"] += tick() - t3
-        it += group_size
-    t_final = tick()
-
-    # Pair counts to the owner of readId0. Owners hold contiguous readId0 ranges (the concatenation of the ranks' candidates
-    # stays sorted), but not equal ones: readId0 < readId1 puts most pairs on low read ids, so the ranges are cut on a
-    # fine histogram (top bits of readId0, summed over the ranks) into groups of equal pair mass.
-    rb = read_bits(read_count_total)
-    fine_bits = max(log2w, min(8, rb))
-    pair_shift = 32 + max(rb - fine_bits, 0)
-    keys, cnts = stages.local_pairs()
-    pk, pv, pc_fine = stages.partition(keys, cnts, pair_shift, fine_bits)
-    pk, pv = pk.clone(), pv.clone()
-    hist = torch.tensor(pc_fine, dtype=torch.int64, device=pk.device)
-    dist.all_reduce(hist, op=dist.ReduceOp.SUM, group=group)
-    bounds = balanced_read_ranges(hist.cpu().numpy(), world)
-    pc = [int(sum(pc_fine[bounds[g]:bounds[g + 1]])) for g in range(world)]
-    rk, _ = all_to_all_v(pk, pc, group)
-    rv, _ = all_to_all_v(pv, pc, group)
-    stages.set_pairs(rk, rv)
-    cand = stages.emit()
-
-    stats = stages.stats_tensor()
-    dist.all_reduce(stats, op=dist.ReduceOp.SUM, group=group)
-    timing["final"] = tick() - t_final
-    return cand, stats, {"log2BucketCount": log2_buckets, "entriesReceived": exchanged, "pairsReceived": int(rk.numel()),
-                         "timing_s": timing}
-
-
-def _exchange_counts(send_counts, group=None):
-    """send_counts[s, d] = items of slab s going to rank d. Returns recv[s, src] = items of slab s coming from src."""
-    world = dist.get_world_size(group)
-    flat = send_counts.t().contiguous().view(-1)             # destination-major: [world, group]
-    out = torch.empty_like(flat)
-    dist.all_to_all_single(out, flat, group=group)           # out[src*group + s] = what src sends me of slab s
-    return out.view(world, -1).t().contiguous()
-
-
-def rebalance_candidates(cand, group=None):
-    """Even out the per-rank candidate slices (owner(readId0) favours low read ids because readId0 < readId1) while
-    keeping the global (rank-order) order: rank g ends up with the g-th contiguous block of the concatenation."""
-    world = dist.get_world_size(group)
-    rank = dist.get_rank(group)
-    dev = torch.device("cuda", torch.cuda.current_device()) if torch.cuda.is_available() and dist.get_backend(group) == "nccl" else torch.device("cpu")
-    n_local = torch.tensor([len(cand)], dtype=torch.int64, device=dev)
-    counts = [torch.zeros(1, dtype=torch.int64, device=dev) for _ in range(world)]
-    dist.all_gather(counts, n_local, group=group)
-    counts = [int(c.item()) for c in counts]
-    total = sum(counts)
-    my_begin = sum(counts[:rank])
-    bounds = [total * g // world for g in range(world + 1)]
-    send = []
-    for g in range(world):
-        lo = min(max(bounds[g], my_begin), my_begin + len(cand))
-        hi = min(max(bounds[g + 1], my_begin), my_begin + len(cand))
-        send.append(hi - lo)
-    t = torch.from_numpy(np.ascontiguousarray(cand, dtype=np.uint32).view(np.int32).reshape(-1)).to(dev)
-    recv, _ = all_to_all_v(t, [3 * x for x in send], group)
-    return recv.cpu().numpy().view(np.uint32).reshape(-1, 3)
-
-
-def gather_candidates(cand, group=None, dst=0):
-    """Concatenate the per-rank candidate slices in rank order on rank `dst` (reference order)."""
-    world = dist.get_world_size(group)
-    rank = dist.get_rank(group)
-    objs = [None] * world if rank == dst else None
-    dist.gather_object(np.ascontiguousarray(cand), objs, dst=dst, group=group)
-    if rank != dst:
-        return None
-    return np.concatenate(objs, axis=0) if objs else np.zeros((0, 3), np.uint32)
-
-
-class _DeviceArray:
-    """Zero-copy view of library-owned device memory for torch (CUDA array interface)."""
-
-    def __init__(self, ptr, n, typestr):
-        self.__cuda_array_interface__ = {"shape": (int(n),), "typestr": typestr, "data": (int(ptr), False), "version": 3}
-
-
-def device_tensor(ptr, n, typestr, device):
-    if n == 0 or not ptr:
-        dtype = {"<i8": torch.int64, "<i4": torch.int32}[typestr]
-        return torch.empty(0, dtype=dtype, device=device)
-    return torch.as_tensor(_DeviceArray(ptr, n, typestr), device=device)
-
-
-class CudaStages:
-    """The per-rank device stages, driven through the C ABI (include/shasta_b200.h, staged LowHash0)."""
-    max_fused_iterations = 16
-
-    def __init__(self, ctx, device):
-        import ctypes as C
-        from . import capi
-        self.C = C
-        self.capi = capi
-        self.ctx = ctx
-        self.device = torch.device("cuda", device) if not isinstance(device, torch.device) else device
-        self.read_count_total = ctx.read_count
-
-    def _check(self, status):
-        self.capi._check(status)
-
-    def begin(self, params):
-        C = self.C
-        self.params = self.capi.make_lowhash_params(**params)
-        log2b = C.c_uint64()
-        self._check(self.capi.lib().shb_lowhash_begin(self.ctx._h, C.byref(self.params), C.byref(log2b)))
-        return int(log2b.value)
-
-    def sweep(self, iteration_begin, count):
-        counts = np.zeros(count, np.uint64)
-        self._check(self.capi.lib().shb_lowhash_sweep(self.ctx._h, iteration_begin, count, counts.ctypes.data))
-        return [int(x) for x in counts]
-
-    def slab(self, s, n):
-        C = self.C
-        k, v = C.c_void_p(), C.c_void_p()
-        self._check(self.capi.lib().shb_lowhash_slab(self.ctx._h, s, C.byref(k), C.byref(v)))
-        return device_tensor(k.value, n, "<i8", self.device), device_tensor(v.value, n, "<i4", self.device)
-
-    def partition(self, keys, vals, shift, bits):
-        C = self.C
-        n = int(keys.numel())
-        counts = np.zeros(1 << bits, np.uint64)
-        ko, vo = C.c_void_p(), C.c_void_p()
-        torch.cuda.synchronize(self.device)
-        self._check(self.capi.lib().shb_device_partition(self.ctx._h, C.c_void_p(keys.data_ptr() if n else 0),
-                                                         C.c_void_p(vals.data_ptr() if n else 0), n, shift, bits,
-                                                         counts.ctypes.data, C.byref(ko), C.byref(vo)))
-        return (device_tensor(ko.value, n, "<i8", self.device), device_tensor(vo.value, n, "<i4", self.device),
-                [int(x) for x in counts])
-
-    def process_entries(self, keys, vals):
-        n = int(keys.numel())
-        torch.cuda.synchronize(self.device)
-        self._check(self.capi.lib().shb_lowhash_process_entries(self.ctx._h, self.C.c_void_p(keys.data_ptr() if n else 0),
-                                                                self.C.c_void_p(vals.data_ptr() if n else 0), n))
-
-    def local_pairs(self):
-        C = self.C
-        k, v, n = C.c_void_p(), C.c_void_p(), C.c_uint64()
-        self._check(self.capi.lib().shb_lowhash_local_pairs(self.ctx._h, C.byref(k), C.byref(v), C.byref(n)))
-        return device_tensor(k.value, n.value, "<i8", self.device), device_tensor(v.value, n.value, "<i4", self.device)
-
-    def set_pairs(self, keys, counts):
-        n = int(keys.numel())
-        torch.cuda.synchronize(self.device)
-        self._check(self.capi.lib().shb_lowhash_set_pairs(self.ctx._h, self.C.c_void_p(keys.data_ptr() if n else 0),
-                                                          self.C.c_void_p(counts.data_ptr() if n else 0), n))
-
-    def emit(self):
-        C = self.C
-        cand, n = C.c_void_p(), C.c_uint64()
-        self._check(self.capi.lib().shb_lowhash_emit(self.ctx._h, C.byref(cand), C.byref(n)))
-        out = self.capi._records_to_array(cand, n.value)        # owns the buffer (shb_free when collected)
-        return out
-
-    def stats_tensor(self):
-        C = self.C
-        p = C.c_void_p()
-        self._check(self.capi.lib().shb_lowhash_stats_device(self.ctx._h, C.byref(p)))
-        return device_tensor(p.value, 3 * self.read_count_total, "<i8", self.device)
-
-    def counters(self):
-        res = self.capi.LowHashResult()
-        self._check(self.capi.lib().shb_lowhash_counters(self.ctx._h, self.C.byref(res)))
-        return res
-
-
-def all_gather_markers(ctx, device, local_toc, group=None):
-    """Replicate the k-mer id rows on every GPU (NCCL all-gather of the shards) for the alignment step.
-    local_toc: this rank's relative toc (2*nLocal+1). Returns (full toc uint64[2R+1], gathered int32 tensor)."""
-    import ctypes as C
-    from . import capi
-    world = dist.get_world_size(group)
-    p, n = C.c_void_p(), C.c_uint64()
-    capi._check(capi.lib().shb_markers_device(ctx._h, C.byref(p), C.byref(n)))
-    dev = torch.device("cuda", device) if not isinstance(device, torch.device) else device
-    local = device_tensor(p.value, n.value, "<i4", dev)
-    sizes = [None] * world
-    dist.all_gather_object(sizes, (int(n.value), np.asarray(local_toc, np.uint64)), group=group)
-    counts = [s[0] for s in sizes]
-    out = torch.empty(sum(counts), dtype=torch.int32, device=dev)
-    chunks = list(out.split(counts))
-    torch.cuda.synchronize(dev)
-    dist.all_gather(chunks, local.contiguous(), group=group) if len(set(counts)) == 1 else _all_gather_v(chunks, local, group)
-    toc = [np.zeros(1, np.uint64)]
-    base = 0
-    for cnt, t in sizes:
-        toc.append(t[1:] + np.uint64(base))
-        base += cnt
-    return np.concatenate(toc), out
-
-
-def _all_gather_v(chunks, local, group):
-    world = dist.get_world_size(group)
-    rank = dist.get_rank(group)
-    for src in range(world):
-        buf = chunks[src]
-        if src == rank:
-            buf.copy_(local)
-        dist.broadcast(buf, src=dist.get_global_rank(group, src) if group is not None else src, group=group)

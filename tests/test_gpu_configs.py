@@ -2,7 +2,7 @@
 both entry points (LowHash0 then computeAlignments) through the C ABI, bit-exact against the CPU oracle.
   C1 conf/Nanopore-Dec2019.conf      (k 10, MinHash 5/30/5, Align defaults + minAlignedFraction 0.4, method 3)
   C2 conf/Nanopore-May2022.conf      (k 14, MinHash 5/30/5, method 3, ds 0.05, skip/drift/trim 100, minMarkers 10, minFrac 0.1)
-  C3 = C2 sharded (tests/test_distributed_cpu.py, tests/run_distributed_gpu.py)
+  C3 = C2 sharded (tests/test_gpu_distributed.py at world 1, tests/run_distributed_gpu.py on 2+ GPUs)
   C4 conf/Nanopore-UL-May2022.conf   (long reads, MinHash 10/50/5, method 3 and --Align.alignMethod 4)
   C5 conf/HiFi-Oct2021.conf          (low error, hashFraction 0.05, 100 iterations, 10/60/3, skip 6, drift 4, trim 2, 200, 0.97)
 MinHash defaults: m 4, hashFraction 0.01, 10 iterations (src/AssemblerOptions.cpp:327-378)."""
