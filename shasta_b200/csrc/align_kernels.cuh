@@ -1414,143 +1414,139 @@ static __global__ void __launch_bounds__(128) align4MatrixKernel(Align4Args g)
     }
 }
 
-// The rest of the front end on the dense global grid (any number of existing cells): the slow path of kernel 2.
-__device__ __noinline__ void align4GlobalTail(const Align4Args& g, uint32_t p, const Align4Grid& G)
+// Front end, kernel 2 of 2, one warp per candidate: cell flags, forward / backward reachability, components, bands.
+// A true overlap leaves a few cells per grid column (100 - 300 for a pair of ultra-long reads, out of 10^4 - 10^5 grid
+// cells), and the three fixpoints over them are chains of dependent neighbour reads: with the existing cells in shared
+// memory (sorted raster indices, an 8-neighbour slot table built once by binary search, flags, labels) a sweep costs
+// shared-memory latencies instead of global ones. Candidates with more existing cells than fit take the global path.
+// Both paths run the same steps (align4ComponentBands) through a view of where the cells are stored.
+constexpr uint32_t kAlign4SmemCells = 512;
+constexpr uint32_t kAlign4WarpsPerBlock = 2;
+constexpr uint16_t kAlign4NoSlot = 0xffffu;
+
+// A candidate's existing cells as kernel 2 sees them. Cell t of the list in raster order has the id id(t); ids increase
+// in raster order. neighbour(c, k) is the id of the cell at (iX + k % 3 - 1, iY + k / 3 - 1) of cell c, or kNone; a
+// cell that does not exist has flags 0. The flags, the label and the YMax of a component root are stored by id;
+// activeLabel(q) is the label of q if q is active, else kNone.
+// Shared memory: the id is the cell's slot in the sorted list, neighbours come from the slot table (existing cells only).
+struct Align4SharedCells {
+    using Id = uint32_t;
+    static constexpr Id kNone = kAlign4NoSlot;
+    const uint32_t* sRow; const uint16_t (*sNbr)[9]; uint8_t* sFlag; uint16_t* sLabel; uint32_t* sYMax;
+    __device__ Id id(uint32_t t) const { return t; }
+    __device__ uint32_t row(Id c) const { return sRow[c]; }
+    __device__ Id neighbour(Id c, int k) const { return sNbr[c][k]; }
+    __device__ uint8_t& flag(Id c) const { return sFlag[c]; }
+    __device__ uint16_t& label(Id c) const { return sLabel[c]; }
+    __device__ Id activeLabel(Id c) const { return sLabel[c]; }            // inactive cells carry kNone
+    __device__ uint32_t& yMax(Id c) const { return sYMax[c]; }
+};
+// The dense grid in global scratch: the id is the raster index. A cell that does not exist keeps its entry count in
+// counts[], so only an active cell's counts[] is a label.
+struct Align4GridCells {
+    using Id = uint32_t;
+    static constexpr Id kNone = 0xffffffffu;
+    const uint32_t* list; uint32_t nIX, nIY; uint8_t* flags; uint32_t* counts; uint32_t* aux;
+    __device__ Id id(uint32_t t) const { return list[t]; }
+    __device__ uint32_t row(Id c) const { return c / nIX; }
+    __device__ Id neighbour(Id c, int k) const
+    {
+        const int32_t qX = int32_t(c % nIX) + k % 3 - 1, qY = int32_t(c / nIX) + k / 3 - 1;
+        return (uint32_t(qX) >= nIX || uint32_t(qY) >= nIY) ? kNone : uint32_t(qY) * nIX + uint32_t(qX);
+    }
+    __device__ uint8_t& flag(Id c) const { return flags[c]; }
+    __device__ Id& label(Id c) const { return counts[c]; }
+    __device__ Id activeLabel(Id c) const { return (flags[c] & 24) == 24 ? counts[c] : kNone; }
+    __device__ uint32_t& yMax(Id c) const { return aux[c]; }
+};
+
+// forwardSearch (:682-729): a cell is forward accessible (flag 8) if one of its parents (iX - {0,1}, iY - {-1,0,1}) is.
+// backwardSearch (:736-787): a cell is backward accessible (flag 16) if one of its children (iX + {0,1}, iY + {-1,0,1}) is.
+template<bool kForward, class Cells>
+__device__ __forceinline__ void align4Search(const Cells& v, uint32_t n)
 {
+    constexpr uint8_t kBit = kForward ? 8 : 16;
+    for(;;) {
+        bool changed = false;
+        for(uint32_t t = threadIdx.x & 31u; t < n; t += 32) {
+            const typename Cells::Id c = v.id(t);
+            const uint8_t f = v.flag(c);
+            if(f & kBit) continue;
+            bool reach = false;
+#pragma unroll
+            for(int e = 0; e < 5; e++) {
+                constexpr int kParents[5] = {7, 6, 3, 1, 0}, kChildren[5] = {8, 7, 5, 2, 1};
+                const typename Cells::Id q = v.neighbour(c, kForward ? kParents[e] : kChildren[e]);
+                if(q != Cells::kNone && (v.flag(q) & kBit)) reach = true;
+            }
+            if(reach) { v.flag(c) = f | kBit; changed = true; }
+        }
+        __syncwarp();
+        if(!__any_sync(0xffffffffu, changed)) break;
+    }
+}
+
+// Kernel 2 after the cell flags, on the n cells of the view: reachability, components of the active cells, and one band
+// per component into the candidate's bands; componentCount[p] = the number of bands.
+template<class Cells>
+__device__ __forceinline__ void align4ComponentBands(const Cells& v, uint32_t n, const Align4Args& g, uint32_t p, const Align4Grid& G)
+{
+    using Id = typename Cells::Id;
     const unsigned lane = threadIdx.x & 31u;
-    const uint32_t nx = G.nx, nIX = G.nIX, nIY = G.nIY, nCells = G.nCells;
-    uint32_t* counts = g.counts + G.base;
-    uint32_t* aux = g.aux + G.base;
-    uint32_t* list = g.list + G.base;
-    uint8_t* flags = g.flags + G.base;
-    int32_t* bands = g.bands + G.base;
-
-    // createCells (:380-436) + compact list of existing cells in raster order.
-    uint32_t listSize = 0;
-    for(uint32_t i0 = 0; i0 < nCells; i0 += 32) {
-        const uint32_t i = i0 + lane;
-        bool exists = false;
-        if(i < nCells) {
-            const uint32_t cnt = counts[i];
-            exists = cnt > 0 && !(int64_t(cnt) < int64_t(g.minEntryCountPerCell));
-            if(exists) {
-                const uint8_t f = align4CellFlags(g, G, i % nIX, i / nIX);
-                flags[i] = f;
-            }
-        }
-        const unsigned m = __ballot_sync(0xffffffffu, exists);
-        if(exists) list[listSize + __popc(m & ((1u << lane) - 1u))] = i;
-        listSize += __popc(m);
+    align4Search<true>(v, n);
+    // backwardSearch seeds: near right / bottom and forward accessible.
+    for(uint32_t t = lane; t < n; t += 32) {
+        const Id c = v.id(t);
+        const uint8_t f = v.flag(c);
+        if((f & 4) && (f & 8)) v.flag(c) = f | 16;
     }
     __syncwarp();
-
-    // forwardSearch (:682-729): fixpoint of "a cell is forward accessible if a parent is".
-    for(;;) {
-        bool changed = false;
-        for(uint32_t t = lane; t < listSize; t += 32) {
-            const uint32_t i = list[t];
-            uint8_t f = flags[i];
-            if(f & 8) continue;
-            const int32_t iX = int32_t(i % nIX), iY = int32_t(i / nIX);
-            bool reach = false;
-            for(int dY = -1; dY <= 1 && !reach; dY++) {
-                const int32_t pY = iY - dY;
-                if(pY < 0 || pY >= int32_t(nIY)) continue;
-                for(int dX = 0; dX <= 1; dX++) {
-                    if(dX == 0 && dY == 0) continue;
-                    const int32_t pX = iX - dX;
-                    if(pX < 0) continue;
-                    if(flags[uint32_t(pY) * nIX + uint32_t(pX)] & 8) { reach = true; break; }
-                }
-            }
-            if(reach) { flags[i] = f | 8; changed = true; }
-        }
-        __syncwarp();
-        if(!__any_sync(0xffffffffu, changed)) break;
-    }
-    // backwardSearch (:736-787): seeds = near right/bottom and forward accessible.
-    for(uint32_t t = lane; t < listSize; t += 32) {
-        const uint32_t i = list[t];
-        const uint8_t f = flags[i];
-        if((f & 4) && (f & 8)) flags[i] = f | 16;
+    align4Search<false>(v, n);
+    // Connected components of the active cells (8-neighbourhood): min-label propagation. Ids are in raster order, so a
+    // component's label ends up as the id of its first cell in raster order, its root.
+    for(uint32_t t = lane; t < n; t += 32) {
+        const Id c = v.id(t);
+        v.label(c) = ((v.flag(c) & 24) == 24) ? c : Cells::kNone;
+        v.yMax(c) = 0;
     }
     __syncwarp();
     for(;;) {
         bool changed = false;
-        for(uint32_t t = lane; t < listSize; t += 32) {
-            const uint32_t i = list[t];
-            uint8_t f = flags[i];
-            if(f & 16) continue;
-            const int32_t iX = int32_t(i % nIX), iY = int32_t(i / nIX);
-            bool reach = false;
-            // this cell is a backward child of c0 = (iX - dX, iY - dY), dX in {-1,0}, dY in {-1,0,1}
-            for(int dY = -1; dY <= 1 && !reach; dY++) {
-                const int32_t pY = iY - dY;
-                if(pY < 0 || pY >= int32_t(nIY)) continue;
-                for(int dX = -1; dX <= 0; dX++) {
-                    if(dX == 0 && dY == 0) continue;
-                    const int32_t pX = iX - dX;
-                    if(pX >= int32_t(nIX)) continue;
-                    if(flags[uint32_t(pY) * nIX + uint32_t(pX)] & 16) { reach = true; break; }
-                }
+        for(uint32_t t = lane; t < n; t += 32) {
+            const Id c = v.id(t);
+            const Id label = v.label(c);
+            if(label == Cells::kNone) continue;
+            Id best = label;
+#pragma unroll
+            for(int k = 0; k < 9; k++) {
+                if(k == 4) continue;
+                const Id q = v.neighbour(c, k);
+                if(q != Cells::kNone) best = min(best, v.activeLabel(q));     // kNone is the largest value
             }
-            if(reach) { flags[i] = f | 16; changed = true; }
+            if(best < label) { v.label(c) = best; changed = true; }
         }
         __syncwarp();
         if(!__any_sync(0xffffffffu, changed)) break;
     }
-
-    // Connected components of the active cells (8-neighbourhood): min-label propagation; counts[] holds labels.
-    for(uint32_t t = lane; t < listSize; t += 32) {
-        const uint32_t i = list[t];
-        counts[i] = ((flags[i] & 24) == 24) ? i : 0xffffffffu;
-    }
-    __syncwarp();
-    for(;;) {
-        bool changed = false;
-        for(uint32_t t = lane; t < listSize; t += 32) {
-            const uint32_t i = list[t];
-            uint32_t label = counts[i];
-            if(label == 0xffffffffu) continue;
-            const int32_t iX = int32_t(i % nIX), iY = int32_t(i / nIX);
-            uint32_t best = label;
-            for(int dY = -1; dY <= 1; dY++) for(int dX = -1; dX <= 1; dX++) {
-                if(!dX && !dY) continue;
-                const int32_t qX = iX + dX, qY = iY + dY;
-                if(qX < 0 || qY < 0 || qX >= int32_t(nIX) || qY >= int32_t(nIY)) continue;
-                const uint32_t j = uint32_t(qY) * nIX + uint32_t(qX);
-                if((flags[j] & 24) != 24) continue;
-                best = min(best, counts[j]);
-            }
-            if(best < label) { counts[i] = best; changed = true; }
-        }
-        __syncwarp();
-        if(!__any_sync(0xffffffffu, changed)) break;
-    }
-    // Per component: root = the cell whose label is its own raster index = the component's first cell in raster
-    // order, so YMin is the root's row; YMax by atomicMax into aux[root].
-    for(uint32_t t = lane; t < listSize; t += 32) {
-        const uint32_t i = list[t];
-        if(counts[i] == i) aux[i] = i / nIX;
-    }
-    __syncwarp();
-    for(uint32_t t = lane; t < listSize; t += 32) {
-        const uint32_t i = list[t];
-        const uint32_t label = counts[i];
-        if(label != 0xffffffffu && label != i) atomicMax(&aux[label], i / nIX);
+    // YMax per component at its root; the root's own row is its YMin.
+    for(uint32_t t = lane; t < n; t += 32) {
+        const Id c = v.id(t);
+        const Id label = v.label(c);
+        if(label != Cells::kNone) atomicMax(&v.yMax(label), v.row(c));
     }
     __syncwarp();
     // One band per component (:890-934), components in raster order of their first cell; too-wide bands dropped.
+    int32_t* bands = g.bands + G.base;
+    const uint32_t nx = G.nx;
     uint32_t nBands = 0;
-    for(uint32_t t0 = 0; t0 < listSize; t0 += 32) {
+    for(uint32_t t0 = 0; t0 < n; t0 += 32) {
         const uint32_t t = t0 + lane;
         bool emit = false;
         int32_t bandMin = 0, bandMax = 0;
-        if(t < listSize) {
-            const uint32_t i = list[t];
-            if(counts[i] == i) {
-                const uint32_t iYMin = i / nIX, iYMax = aux[i];
-                const uint32_t YMin = iYMin * g.deltaY, YMax = (iYMax + 1) * g.deltaY - 1;
+        if(t < n) {
+            const Id c = v.id(t);
+            if(v.label(c) == c) {
+                const uint32_t YMin = v.row(c) * g.deltaY, YMax = (v.yMax(c) + 1) * g.deltaY - 1;
                 bandMin = int32_t(nx) - 1 - int32_t(YMax);
                 bandMax = int32_t(nx) - 1 - int32_t(YMin);
                 emit = !(int64_t(bandMax - bandMin + 1) > g.maxBand);
@@ -1564,18 +1560,34 @@ __device__ __noinline__ void align4GlobalTail(const Align4Args& g, uint32_t p, c
         }
         nBands += __popc(m);
     }
+    __syncwarp();
     if(lane == 0) g.componentCount[p] = nBands;
 }
 
-
-// Front end, kernel 2 of 2, one warp per candidate: cell flags, forward / backward reachability, components, bands.
-// A true overlap leaves a few cells per grid column (100 - 300 for a pair of ultra-long reads, out of 10^4 - 10^5 grid
-// cells), and the three fixpoints over them are chains of dependent neighbour reads: with the existing cells in shared
-// memory (sorted raster indices, an 8-neighbour slot table built once by binary search, flags, labels) a sweep costs
-// shared-memory latencies instead of global ones. Candidates with more existing cells than fit take the global path.
-constexpr uint32_t kAlign4SmemCells = 512;
-constexpr uint32_t kAlign4WarpsPerBlock = 2;
-constexpr uint16_t kAlign4NoSlot = 0xffffu;
+// Kernel 2 on the dense global grid (any number of existing cells): createCells (:380-436) writes the flags, and a scan
+// of the grid lists the existing cells in raster order. Out of line, so that the shared-memory path keeps its registers.
+__device__ __noinline__ void align4GridComponents(const Align4Args& g, uint32_t p, const Align4Grid& G)
+{
+    const unsigned lane = threadIdx.x & 31u;
+    const uint32_t nCells = G.nCells;
+    uint32_t* list = g.list + G.base;
+    const Align4GridCells v{list, G.nIX, G.nIY, g.flags + G.base, g.counts + G.base, g.aux + G.base};
+    uint32_t listSize = 0;
+    for(uint32_t i0 = 0; i0 < nCells; i0 += 32) {
+        const uint32_t i = i0 + lane;
+        bool exists = false;
+        if(i < nCells) {
+            const uint32_t cnt = v.counts[i];
+            exists = cnt > 0 && !(int64_t(cnt) < int64_t(g.minEntryCountPerCell));
+            if(exists) v.flags[i] = align4CellFlags(g, G, i % G.nIX, i / G.nIX);
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, exists);
+        if(exists) list[listSize + __popc(m & ((1u << lane) - 1u))] = i;
+        listSize += __popc(m);
+    }
+    __syncwarp();
+    align4ComponentBands(v, listSize, g, p, G);
+}
 
 static __global__ void __launch_bounds__(kAlign4WarpsPerBlock * 32) align4ComponentsKernel(Align4Args g, uint32_t smemCells)
 {
@@ -1590,7 +1602,7 @@ static __global__ void __launch_bounds__(kAlign4WarpsPerBlock * 32) align4Compon
     const Align4Grid G = align4Grid(g, p);
     if(G.nCells == 0) { if(lane == 0) g.componentCount[p] = 0; return; }
     const uint32_t n = g.componentCount[p];                 // existing cells (kernel 1)
-    if(n > smemCells) { align4GlobalTail(g, p, G); return; }
+    if(n > smemCells) { align4GridComponents(g, p, G); return; }
     if(n == 0) return;                                      // no cells, no components: componentCount[p] is already 0
     uint32_t* sIdx = sIdxAll[warp]; uint32_t* sYMax = sYMaxAll[warp];
     uint16_t (*sNbr)[9] = sNbrAll[warp]; uint16_t* sLabel = sLabelAll[warp]; uint8_t* sFlag = sFlagAll[warp];
@@ -1638,98 +1650,7 @@ static __global__ void __launch_bounds__(kAlign4WarpsPerBlock * 32) align4Compon
     __syncwarp();
     for(uint32_t t = lane; t < n; t += 32) sIdx[t] /= nIX;          // from here on only the row is needed
     __syncwarp();
-
-    // forwardSearch (:682-729): a cell is forward accessible if one of its parents (iX - {0,1}, iY - {-1,0,1}) is.
-    for(;;) {
-        bool changed = false;
-        for(uint32_t t = lane; t < n; t += 32) {
-            const uint8_t f = sFlag[t];
-            if(f & 8) continue;
-            bool reach = false;
-#pragma unroll
-            for(int e = 0; e < 5; e++) {
-                constexpr int kParents[5] = {7, 6, 3, 1, 0};
-                const uint16_t q = sNbr[t][kParents[e]];
-                if(q != kAlign4NoSlot && (sFlag[q] & 8)) reach = true;
-            }
-            if(reach) { sFlag[t] = f | 8; changed = true; }
-        }
-        __syncwarp();
-        if(!__any_sync(0xffffffffu, changed)) break;
-    }
-    // backwardSearch (:736-787): seeds = near right / bottom and forward accessible; then through the children.
-    for(uint32_t t = lane; t < n; t += 32) {
-        const uint8_t f = sFlag[t];
-        if((f & 4) && (f & 8)) sFlag[t] = f | 16;
-    }
-    __syncwarp();
-    for(;;) {
-        bool changed = false;
-        for(uint32_t t = lane; t < n; t += 32) {
-            const uint8_t f = sFlag[t];
-            if(f & 16) continue;
-            bool reach = false;
-#pragma unroll
-            for(int e = 0; e < 5; e++) {
-                constexpr int kChildren[5] = {8, 7, 5, 2, 1};
-                const uint16_t q = sNbr[t][kChildren[e]];
-                if(q != kAlign4NoSlot && (sFlag[q] & 16)) reach = true;
-            }
-            if(reach) { sFlag[t] = f | 16; changed = true; }
-        }
-        __syncwarp();
-        if(!__any_sync(0xffffffffu, changed)) break;
-    }
-    // Connected components of the active cells (8-neighbourhood): min-label propagation over the slots. Slots are in
-    // raster order, so a component's label ends up as the slot of its first cell in raster order.
-    for(uint32_t t = lane; t < n; t += 32) { sLabel[t] = ((sFlag[t] & 24) == 24) ? uint16_t(t) : kAlign4NoSlot; sYMax[t] = 0; }
-    __syncwarp();
-    for(;;) {
-        bool changed = false;
-        for(uint32_t t = lane; t < n; t += 32) {
-            const uint16_t label = sLabel[t];
-            if(label == kAlign4NoSlot) continue;
-            uint16_t best = label;
-#pragma unroll
-            for(int k = 0; k < 9; k++) {
-                if(k == 4) continue;
-                const uint16_t q = sNbr[t][k];
-                if(q != kAlign4NoSlot) best = min(best, sLabel[q]);     // inactive neighbours carry kAlign4NoSlot = the largest value
-            }
-            if(best < label) { sLabel[t] = best; changed = true; }
-        }
-        __syncwarp();
-        if(!__any_sync(0xffffffffu, changed)) break;
-    }
-    for(uint32_t t = lane; t < n; t += 32) {
-        const uint16_t label = sLabel[t];
-        if(label != kAlign4NoSlot) atomicMax(&sYMax[label], sIdx[t]);
-    }
-    __syncwarp();
-    // One band per component (:890-934), components in raster order of their first cell; too-wide bands dropped.
-    int32_t* bands = g.bands + G.base;
-    const uint32_t nx = G.nx;
-    uint32_t nBands = 0;
-    for(uint32_t t0 = 0; t0 < n; t0 += 32) {
-        const uint32_t t = t0 + lane;
-        bool emit = false;
-        int32_t bandMin = 0, bandMax = 0;
-        if(t < n && sLabel[t] == uint16_t(t)) {
-            const uint32_t YMin = sIdx[t] * g.deltaY, YMax = (sYMax[t] + 1) * g.deltaY - 1;
-            bandMin = int32_t(nx) - 1 - int32_t(YMax);
-            bandMax = int32_t(nx) - 1 - int32_t(YMin);
-            emit = !(int64_t(bandMax - bandMin + 1) > g.maxBand);
-        }
-        const unsigned m = __ballot_sync(0xffffffffu, emit);
-        if(emit) {
-            const uint32_t slot = nBands + __popc(m & ((1u << lane) - 1u));
-            bands[2 * slot] = bandMin;
-            bands[2 * slot + 1] = bandMax;
-        }
-        nBands += __popc(m);
-    }
-    __syncwarp();
-    if(lane == 0) g.componentCount[p] = nBands;
+    align4ComponentBands(Align4SharedCells{sIdx, sNbr, sFlag, sLabel, sYMax}, n, g, p, G);
 }
 
 // Expand (candidate, component) into DP jobs. jobOffsets = exclusive scan of componentCount.
