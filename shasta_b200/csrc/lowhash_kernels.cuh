@@ -155,13 +155,7 @@ static __global__ void sweepTileReadsKernel(const uint64_t* __restrict__ toc, ui
 {
     const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if(t >= tileCount) return;
-    const uint64_t p = uint64_t(t) * kSweepTile;
-    uint32_t lo = 0, hi = orientedReadCount;            // largest lo with toc[lo] <= p (toc[0] = 0)
-    while(hi - lo > 1) {
-        const uint32_t mid = lo + ((hi - lo) >> 1);
-        if(toc[mid] <= p) lo = mid; else hi = mid;
-    }
-    tileFirstRead[t] = lo;
+    tileFirstRead[t] = rowOf(toc, 0u, orientedReadCount, uint64_t(t) * kSweepTile);         // toc[0] = 0
 }
 
 // Which oriented read does marker position p belong to, and is the feature starting at p valid
@@ -169,11 +163,7 @@ static __global__ void sweepTileReadsKernel(const uint64_t* __restrict__ toc, ui
 // oriented read index or 0xffffffff.
 __device__ __forceinline__ uint32_t resolveFeature(const SweepArgs& a, uint64_t p, uint32_t m)
 {
-    uint32_t lo = 0, hi = a.orientedReadCount;          // largest lo with toc[lo] <= p
-    while(hi - lo > 1) {
-        const uint32_t mid = lo + ((hi - lo) >> 1);
-        if(a.toc[mid] <= p) lo = mid; else hi = mid;
-    }
+    const uint32_t lo = rowOf(a.toc, 0u, a.orientedReadCount, p);
     const bool inside = (p + m <= a.toc[lo + 1]);
     const bool palindromic = (a.readFlags[(a.orientedReadBase + lo) >> 1] & 1u) != 0;
     return (inside && !palindromic) ? lo : 0xffffffffu;

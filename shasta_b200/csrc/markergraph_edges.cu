@@ -57,7 +57,7 @@ __global__ void __launch_bounds__(kMgThreads) successorKernel(const uint64_t* __
         const uint64_t m0 = markers[i];
         if(m0 >= M) { atomicMin(scal + 0, (unsigned long long)i); targets[i] = kInvalid40; continue; }
         if(i > b && markers[i - 1] >= m0) atomicMin(scal + 1, (unsigned long long)i);
-        const uint32_t o = orientedReadOf(toc, rows, m0);
+        const uint32_t o = rowOf(toc, 0u, rows, m0);
         const uint64_t first = toc[o], end = toc[o + 1];
         uint64_t t = kInvalid40, m = m0 + 1;
         for(uint32_t k = 0; k < kShortWalk && m < end; k++, m++) {

@@ -1,5 +1,6 @@
 // Device helpers shared by the marker graph vertices (markergraph.cu) and edges (markergraph_edges.cu): Uint40 loads and
-// stores, the oriented read of a marker, and the segmented rank sorts of distinct uint64 keys.
+// stores, the reverse complement of a marker, and the segmented rank sorts of distinct uint64 keys. The oriented read of a
+// marker is rowOf (primitives.cuh).
 #pragma once
 
 #include "context.cuh"
@@ -66,17 +67,9 @@ __device__ __forceinline__ uint64_t load40(const uint8_t* p)
     return v;
 }
 
-// shasta::findMarkerId: the oriented read of marker m, the last row whose first marker is <= m (a non-empty row).
-__device__ __forceinline__ uint32_t orientedReadOf(const uint64_t* __restrict__ toc, uint32_t rows, uint64_t m)
-{
-    uint32_t lo = 0, hi = rows;
-    while(hi - lo > 1) { const uint32_t mid = lo + ((hi - lo) >> 1); if(toc[mid] <= m) lo = mid; else hi = mid; }
-    return lo;
-}
-
 __device__ __forceinline__ uint64_t reverseComplementMarker(const uint64_t* __restrict__ toc, uint32_t rows, uint64_t m)
 {
-    const uint32_t lo = orientedReadOf(toc, rows, m);
+    const uint32_t lo = rowOf(toc, 0u, rows, m);
     const uint64_t ordinal = m - toc[lo], size = toc[lo + 1] - toc[lo];
     return toc[lo ^ 1u] + (size - 1 - ordinal);
 }

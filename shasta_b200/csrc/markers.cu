@@ -23,16 +23,6 @@ extern thread_local uint64_t g_launchCount;
 
 namespace {
 
-__device__ __forceinline__ uint32_t reverseComplementKmer(uint32_t kmer, uint32_t k)
-{
-    // bit-plane reverse complement: complement = invert both planes, reverse = bit-reverse each k-bit plane
-    // (src/ShortBaseSequence.hpp:109-118, src/Base.hpp:139-143)
-    const uint32_t mask = (k == 16) ? 0xffffu : ((1u << k) - 1u);
-    const uint32_t lsb = ~kmer & mask;
-    const uint32_t msb = ~(kmer >> k) & mask;
-    return ((__brev(msb) >> (32 - k)) << k) | (__brev(lsb) >> (32 - k));
-}
-
 // The read a 64-base block belongs to: largest r with blockStart[r] <= g (blockStart = word offsets / 2).
 __device__ __forceinline__ uint32_t readOfBlock(const uint64_t* __restrict__ wordOffsets, uint32_t readCount, uint64_t g)
 {

@@ -12,30 +12,21 @@
 
 #include <chrono>
 #include <cstring>
+#include <functional>
 #include <vector>
 
 namespace shb {
 
 extern thread_local uint64_t g_launchCount;
 
+void sortMarkersByKmer(shb_context* c, uint32_t rowStep, uint64_t chunkLimit, uint32_t kmerBits, const char* tooLong,
+                       const std::function<void(const uint64_t*, const uint32_t*, uint32_t, uint32_t, uint64_t, uint32_t)>& sorted);
+
 namespace {
 
 using namespace pal;
 
 // ---- phase A -------------------------------------------------------------------------------------------------------
-__global__ void palKeysKernel(const uint32_t* __restrict__ kmerIds, const uint64_t* __restrict__ toc, uint32_t rowBegin,
-                              uint32_t rowEnd, uint64_t markerBegin, uint32_t n, uint64_t* __restrict__ keys,
-                              uint32_t* __restrict__ ordinals)
-{
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if(i >= n) return;
-    const uint64_t p = markerBegin + i;
-    uint32_t lo = rowBegin, hi = rowEnd;            // largest row with toc[row] <= p
-    while(hi - lo > 1) { const uint32_t mid = lo + ((hi - lo) >> 1); if(toc[mid] <= p) lo = mid; else hi = mid; }
-    keys[i] = (uint64_t(lo - rowBegin) << 32) | kmerIds[p];
-    ordinals[i] = uint32_t(p - toc[lo]);
-}
-
 // One thread per read: the merge join of createVertices (src/AlignmentGraph.cpp:179-249), counting only.
 __global__ void palPrefilterKernel(const uint64_t* __restrict__ keys, const uint32_t* __restrict__ ordinals,
                                    const uint64_t* __restrict__ toc, uint64_t readBegin, uint64_t readEnd, uint64_t markerBegin,
@@ -382,35 +373,16 @@ void flagPalindromicReads(shb_context* c, const shb_palindromic_params& p, uint8
     DeviceBuffer<uint8_t> survives;
     vBound.reserve(R + 1); vNearBound.reserve(R + 1); survives.reserve(R + 1);
 
-    // Phase A, in chunks of whole reads (SHB_PALINDROMIC_SORT_CHUNK markers: test hook).
-    const std::vector<uint64_t>& toc = c->tocHost;
+    // Phase A, in chunks of whole reads (SHB_PALINDROMIC_SORT_CHUNK markers: test hook), so that strand 0 of each read is
+    // merge-joined against strand 1 inside one chunk.
     const uint64_t chunkLimit = envCount("SHB_PALINDROMIC_SORT_CHUNK", 1u << 28);
-    DeviceBuffer<uint64_t> keysA, keysB;
-    DeviceBuffer<uint32_t> valsA, valsB;
-    for(uint64_t readBegin = 0; readBegin < R; ) {
-        uint64_t readEnd = readBegin + 1;
-        while(readEnd < R && toc[2 * (readEnd + 1)] - toc[2 * readBegin] <= chunkLimit) readEnd++;
-        const uint64_t markerBegin = toc[2 * readBegin];
-        const uint64_t n64 = toc[2 * readEnd] - markerBegin;
-        SHB_REQUIRE(n64 < (1ull << 32), SHB_ERR_INVALID, "A read has more than 2^32-1 markers.");
-        const uint32_t n = uint32_t(n64);
-        const uint32_t rowBegin = uint32_t(2 * readBegin), rowEnd = uint32_t(2 * readEnd);
-        const uint64_t* keys = nullptr; const uint32_t* vals = nullptr;
-        if(n) {
-            keysA.reserve(n); keysB.reserve(n); valsA.reserve(n); valsB.reserve(n);
-            SHB_LAUNCH(palKeysKernel, ceilDiv(n, 256), 256, 0, st, c->kmerIds, (const uint64_t*)c->toc.get(), rowBegin, rowEnd,
-                       markerBegin, n, keysA.get(), valsA.get());
-            const uint32_t rowBits = bitsFor(rowEnd - rowBegin - 1);
-            const int ranges[2][2] = {{0, 32}, {32, 32 + int(rowBits)}};
-            const bool inB = radixSort<true>(keysA.get(), keysB.get(), valsA.get(), valsB.get(), n, ranges, 2, c->sortWs, st);
-            keys = inB ? keysB.get() : keysA.get();
-            vals = inB ? valsB.get() : valsA.get();
-        }
+    sortMarkersByKmer(c, 2, chunkLimit, 32, "A read has more than 2^32-1 markers.",
+                      [&](const uint64_t* keys, const uint32_t* vals, uint32_t rowBegin, uint32_t rowEnd, uint64_t markerBegin, uint32_t) {
+        const uint64_t readBegin = rowBegin / 2, readEnd = rowEnd / 2;
         SHB_LAUNCH(palPrefilterKernel, ceilDiv(readEnd - readBegin, 128), 128, 0, st, keys, vals, (const uint64_t*)c->toc.get(),
                    readBegin, readEnd, markerBegin, p.maxMarkerFrequency, p.deltaThreshold, p.alignedFractionThreshold,
                    p.nearDiagonalFractionThreshold, vBound.get(), vNearBound.get(), survives.get());
-        readBegin = readEnd;
-    }
+    });
     std::vector<uint64_t> vb(R), vnb(R);
     std::vector<uint8_t> sv(R);
     if(R) {
@@ -419,7 +391,6 @@ void flagPalindromicReads(shb_context* c, const shb_palindromic_params& p, uint8
         SHB_CUDA(cudaMemcpyAsync(sv.data(), survives.get(), R, cudaMemcpyDeviceToHost, st));
     }
     SHB_CUDA(cudaStreamSynchronize(st));
-    keysA.release(); keysB.release(); valsA.release(); valsB.release();
 
     // Phase B.
     const auto t1 = std::chrono::steady_clock::now();

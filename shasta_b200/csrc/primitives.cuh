@@ -1,5 +1,6 @@
 // Hand-written device-wide primitives used by the LowHash and alignment pipelines:
-// exclusive scan, stream compaction helpers, and (radix_sort.cuh) the LSD radix sort.
+// exclusive scan, stream compaction helpers, (radix_sort.cuh) the LSD radix sort, row starts and the row search that
+// inverts them, and the k-mer id reverse complement.
 // All are plain sm_90a CUDA (warp shuffles / match_any / shared-memory atomics); no CUB/Thrust.
 #pragma once
 
@@ -153,6 +154,24 @@ template<class T> __global__ void rowStartsKernel(const uint64_t* __restrict__ s
     uint32_t lo = 0, hi = entries;
     while(lo < hi) { const uint32_t mid = lo + ((hi - lo) >> 1); if(uint32_t(sortedKeys[mid] >> 32) < row) lo = mid + 1; else hi = mid; }
     toc[row] = T(lo);
+}
+
+// The inverse of rowStartsKernel: the last row r in [lo, hi) with toc[r] <= p, for a non-decreasing toc with toc[lo] <= p.
+// For the marker toc this is the oriented read of marker position p (shasta::findMarkerId); empty rows are skipped.
+template<class T, class P> __device__ __forceinline__ uint32_t rowOf(const T* toc, uint32_t lo, uint32_t hi, P p)
+{
+    while(hi - lo > 1) { const uint32_t mid = lo + ((hi - lo) >> 1); if(toc[mid] <= p) lo = mid; else hi = mid; }
+    return lo;
+}
+
+// The reverse complement of a k-mer id (k <= 16). Bit-plane reverse complement: complement = invert both planes, reverse =
+// bit-reverse each k-bit plane (src/ShortBaseSequence.hpp:109-118, src/Base.hpp:139-143).
+__device__ __forceinline__ uint32_t reverseComplementKmer(uint32_t kmer, uint32_t k)
+{
+    const uint32_t mask = (k == 16) ? 0xffffu : ((1u << k) - 1u);
+    const uint32_t lsb = ~kmer & mask;
+    const uint32_t msb = ~(kmer >> k) & mask;
+    return ((__brev(msb) >> (32 - k)) << k) | (__brev(lsb) >> (32 - k));
 }
 
 // out[i] = in[i] widened to 64 bits, for i < n. N, the index type, is uint32_t or uint64_t.

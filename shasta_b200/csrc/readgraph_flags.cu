@@ -260,8 +260,7 @@ __global__ void adjacencyKernel(const uint32_t* __restrict__ toc, uint32_t rows,
 {
     const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
     if(p >= entries) return;
-    uint32_t lo = 0, hi = rows;                 // the last row whose toc is <= p
-    while(hi - lo > 1) { const uint32_t mid = lo + ((hi - lo) >> 1); if(toc[mid] <= p) lo = mid; else hi = mid; }
+    const uint32_t lo = rowOf(toc, 0u, rows, p);
     const uint32_t e = data[p];
     if(e >= edgeCount) { atomicAdd(bad, 1u); adj[p] = 0; return; }
     const uint32_t w0 = edges[4ull * e], w1 = edges[4ull * e + 1], flags = edges[4ull * e + 3];

@@ -17,14 +17,6 @@ __host__ __device__ inline uint64_t mix64(uint64_t seed, uint64_t stream, uint64
 }
 __device__ inline double unitOf(uint64_t x) { return double(x >> 11) * (1.0 / 9007199254740992.0); }
 
-__device__ inline uint32_t reverseComplementKmer(uint32_t kmer, uint32_t k)
-{
-    const uint32_t mask = (k == 16) ? 0xffffu : ((1u << k) - 1u);
-    const uint32_t lsb = ~kmer & mask;
-    const uint32_t msb = ~(kmer >> k) & mask;
-    return ((__brev(msb) >> (32 - k)) << k) | (__brev(lsb) >> (32 - k));
-}
-
 struct SynthArgs {
     uint64_t seed; uint32_t k; double drop; double ins;
     const uint32_t* genomeKmer; const uint64_t* genomePos;
