@@ -59,6 +59,18 @@ def recorded(group, key, fn, *args, **kwargs):
             atexit.register(_save)
         _pending.setdefault(group, {})[key] = value
         return value
+    return _stored(group, key)
+
+
+def stored(group, key):
+    """The value under `key` without calling the reference: the one recorded in this process under
+    SHB_RECORD_REFERENCE=1, else the one in the file."""
+    if key in _pending.get(group, {}):
+        return _pending[group][key]
+    return _stored(group, key)
+
+
+def _stored(group, key):
     if group not in _loaded:
         with np.load(_path(group)) as z:
             _loaded[group] = dict(z)
