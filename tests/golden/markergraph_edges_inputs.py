@@ -7,6 +7,7 @@ import hashlib
 import numpy as np
 
 from oracle import markergraph_bindings as MB
+from oracle import markergraph_edges_bindings as EB
 
 from markergraph_inputs import PARAMS, cases
 
@@ -118,3 +119,37 @@ def digest(*arrays):
     for a in arrays:
         h.update(np.ascontiguousarray(a).tobytes())
     return np.frombuffer(h.digest(), np.uint8)
+
+
+def parallel_edge(s, e):
+    """Edge e duplicated at the end of the edge list, with its intervals, and listed in its source's row: parallel edges."""
+    s = {k: np.array(v) for k, v in s.items() if isinstance(v, np.ndarray)}
+    E = len(s["edges"])
+    itoc = s["intervalsToc"].astype(np.int64)
+    s["edges"] = np.concatenate([s["edges"], s["edges"][e:e + 1]])
+    s["intervalsData"] = np.concatenate([s["intervalsData"], s["intervalsData"][itoc[e]:itoc[e + 1]]])
+    s["intervalsToc"] = np.append(s["intervalsToc"], s["intervalsToc"][-1] + (itoc[e + 1] - itoc[e])).astype(np.uint64)
+    src = int(EB.named_fields(s["edges"][e:e + 1])[0, 0])
+    stoc = s["bySourceToc"].astype(np.int64)
+    data = list(s["bySourceData"].tolist())
+    data.insert(stoc[src], E)                            # the new id first: rows are in decreasing edge id
+    s["bySourceData"] = np.array(data, np.uint64)
+    s["bySourceToc"][src + 1:] += 1
+    return s
+
+
+def drop_interval(s, e):
+    """Edge e without its last interval."""
+    s = {k: np.array(v) for k, v in s.items() if isinstance(v, np.ndarray)}
+    itoc = s["intervalsToc"].astype(np.int64)
+    s["intervalsData"] = np.delete(s["intervalsData"], itoc[e + 1] - 1, axis=0)
+    s["intervalsToc"][e + 1:] -= 1
+    return s
+
+
+def rc_failure_inputs(d):
+    """(name, vertices d, edge set) for the two failures the reference reports, on the edges of the vertices d."""
+    o = EB.oracle_create_marker_graph_edges(d["toc"], d["table"], d["vtoc"], d["vdata"])
+    cov = np.diff(o["intervalsToc"].astype(np.int64))
+    e = int(np.nonzero(cov >= 2)[0][3])
+    return [("missing_interval", d, drop_interval(o, e)), ("parallel", d, parallel_edge(o, e))]

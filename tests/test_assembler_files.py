@@ -10,7 +10,6 @@ sequence (scripts/FindAlignmentCandidatesLowHash0.py, scripts/ComputeAlignments.
 import gzip
 import hashlib
 import os
-import sys
 
 import numpy as np
 import pytest
@@ -18,8 +17,8 @@ import pytest
 from oracle import bindings as B
 from shasta_b200 import assembler as A
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
-from reference_outputs import recorded  # noqa: E402
+import support  # noqa: F401  (puts tests/golden on sys.path)
+from reference_outputs import recorded
 
 
 def fnv(raw):

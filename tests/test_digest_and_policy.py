@@ -5,6 +5,7 @@ restatement of src/AssemblerAlignmentCandidates.cpp:379-448."""
 import numpy as np
 
 from oracle import bindings as B
+from support import candidate_set
 
 M64 = (1 << 64) - 1
 FNV_OFFSET, FNV_PRIME = 0xcbf29ce484222325, 0x100000001b3
@@ -91,11 +92,7 @@ def test_every_policy_gives_an_optimal_path_of_the_same_score():
 
 def test_tie_flags_bound_the_policy_exposure():
     # A candidate whose tie flags are clear has a unique optimum: every policy must return the same alignment.
-    from shasta_b200 import synth
-    p = synth.SynthParams(reads=150, k=10, genome_markers=12000, n50_bases=12000, min_bases=6000, seed=11)
-    d = synth.generate(p)
-    lp = B.LowHashParams(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2, maxBucketSize=30, minFrequency=2)
-    cand, _, _ = B.oracle_lowhash0(d["toc"], d["data"], d["flags"], lp)
+    d, cand = candidate_set(150, 10, 11, genome_markers=12000, n50=12000, min_bases=6000)
     cand = cand[:400]
     oo = B.make_align_options(alignMethod=3, k=10, minAlignedMarkerCount=30, minAlignedFraction=0.2)
     default = B.default_dp_policy()

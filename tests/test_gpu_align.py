@@ -5,98 +5,64 @@ import numpy as np
 import pytest
 
 from oracle import bindings as B
-from shasta_b200 import synth
+from support import candidate_set, compare_alignments, ctx  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
 
-@pytest.fixture(scope="module")
-def ctx():
-    from shasta_b200 import capi
-    c = capi.Context(0)
-    yield c
-    c.close()
-
-
-def _dataset(reads, k, seed, **kw):
-    p = synth.SynthParams(reads=reads, k=k, genome_markers=kw.pop("genome_markers", 20000), n50_bases=kw.pop("n50", 15000),
-                          min_bases=kw.pop("min_bases", 8000), seed=seed, **kw)
-    d = synth.generate(p)
-    lp = B.LowHashParams(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2, maxBucketSize=30, minFrequency=2)
-    cand, _, _ = B.oracle_lowhash0(d["toc"], d["data"], d["flags"], lp)
-    return d, cand
-
-
-def _compare(ctx, d, cand, **opts):
-    from shasta_b200 import capi
-    ctx.set_markers(d["toc"], d["data"], d["flags"])
-    go = capi.make_align_options(**opts)
-    rec, ctoc, cdata, res = capi.compute_alignments(ctx, cand, go)
-    oo = B.make_align_options(**{k: v for k, v in opts.items() if k in B.ALIGN_DEFAULTS})
-    orec, otoc, odata, _ = B.oracle_compute_alignments(d["toc"], d["kmer"], cand, oo, threads=8)
-    assert res.candidateCount == len(cand)
-    assert rec.shape == orec.shape, (rec.shape, orec.shape)
-    assert np.array_equal(rec, orec)
-    assert np.array_equal(ctoc, otoc)
-    assert np.array_equal(cdata, odata)
-    # the device-side digests carried by every bench line are those of exactly these bytes
-    assert res.alignmentDataDigest == capi.digest_records(orec, 16)
-    assert res.compressedDigest == capi.digest_compressed(orec, otoc, odata)
-    assert res.dpUsefulCells <= res.dpCells
-    return rec, res
-
-
 def test_method3_nanopore_like(ctx):
-    d, cand = _dataset(300, 10, 5)
-    rec, res = _compare(ctx, d, cand[:1500], alignMethod=3, k=10, maxSkip=30, maxDrift=30, maxTrim=30,
-                        minAlignedMarkerCount=100, minAlignedFraction=0.4, downsamplingFactor=0.1, bandExtend=10, maxBand=1000)
+    d, cand = candidate_set(300, 10, 5)
+    rec, _, _, res = compare_alignments(ctx, d, cand[:1500], alignMethod=3, k=10, maxSkip=30, maxDrift=30, maxTrim=30,
+                                        minAlignedMarkerCount=100, minAlignedFraction=0.4, downsamplingFactor=0.1,
+                                        bandExtend=10, maxBand=1000)
     assert len(rec) > 100 and res.dpCells > 0
 
 
 def test_method3_may2022_options(ctx):
-    d, cand = _dataset(250, 14, 9)
-    rec, _ = _compare(ctx, d, cand[:1200], alignMethod=3, k=14, maxSkip=100, maxDrift=100, maxTrim=100,
-                      minAlignedMarkerCount=10, minAlignedFraction=0.1, downsamplingFactor=0.05, bandExtend=10, maxBand=1000)
+    d, cand = candidate_set(250, 14, 9)
+    rec = compare_alignments(ctx, d, cand[:1200], alignMethod=3, k=14, maxSkip=100, maxDrift=100, maxTrim=100,
+                             minAlignedMarkerCount=10, minAlignedFraction=0.1, downsamplingFactor=0.05, bandExtend=10,
+                             maxBand=1000)[0]
     assert len(rec) > 100
 
 
 def test_method3_strict_filters_and_containments(ctx):
-    d, cand = _dataset(250, 14, 13, drop=0.02, ins=0.01)
-    _compare(ctx, d, cand[:1000], alignMethod=3, k=14, maxSkip=6, maxDrift=4, maxTrim=2, minAlignedMarkerCount=200,
-             minAlignedFraction=0.97, downsamplingFactor=0.05, bandExtend=10, maxBand=1000)
-    _compare(ctx, d, cand[:1000], alignMethod=3, k=14, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=50,
-             minAlignedFraction=0.3, downsamplingFactor=0.1, bandExtend=5, maxBand=40, suppressContainments=1)
+    d, cand = candidate_set(250, 14, 13, drop=0.02, ins=0.01)
+    compare_alignments(ctx, d, cand[:1000], alignMethod=3, k=14, maxSkip=6, maxDrift=4, maxTrim=2, minAlignedMarkerCount=200,
+                       minAlignedFraction=0.97, downsamplingFactor=0.05, bandExtend=10, maxBand=1000)
+    compare_alignments(ctx, d, cand[:1000], alignMethod=3, k=14, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=50,
+                       minAlignedFraction=0.3, downsamplingFactor=0.1, bandExtend=5, maxBand=40, suppressContainments=1)
 
 
 def test_method3_random_pairs_and_scores(ctx):
     # Unrelated read pairs (mostly empty / rejected alignments) and non-default scores.
-    d, _ = _dataset(120, 10, 21)
+    d, _ = candidate_set(120, 10, 21)
     rng = np.random.default_rng(3)
     a = rng.integers(0, 119, 600)
     b = rng.integers(0, 119, 600)
     lo, hi = np.minimum(a, b), np.maximum(a, b)
     ok = lo < hi
     cand = np.stack([lo[ok], hi[ok], rng.integers(0, 2, ok.sum())], 1).astype(np.uint32)
-    _compare(ctx, d, cand, alignMethod=3, k=10, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=5,
-             minAlignedFraction=0.05, downsamplingFactor=0.2, bandExtend=10, maxBand=1000)
-    _compare(ctx, d, cand, alignMethod=3, k=10, maxSkip=50, maxDrift=50, maxTrim=1000, minAlignedMarkerCount=3,
-             minAlignedFraction=0.0, matchScore=3, mismatchScore=-2, gapScore=-1, downsamplingFactor=0.3,
-             bandExtend=3, maxBand=200)
+    compare_alignments(ctx, d, cand, alignMethod=3, k=10, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=5,
+                       minAlignedFraction=0.05, downsamplingFactor=0.2, bandExtend=10, maxBand=1000)
+    compare_alignments(ctx, d, cand, alignMethod=3, k=10, maxSkip=50, maxDrift=50, maxTrim=1000, minAlignedMarkerCount=3,
+                       minAlignedFraction=0.0, matchScore=3, mismatchScore=-2, gapScore=-1, downsamplingFactor=0.3,
+                       bandExtend=3, maxBand=200)
 
 
 def test_method1_unbanded_all_markers(ctx):
     # Align.alignMethod 1 (src/AssemblerAlign1.cpp:129-148): one unbanded DP on all markers; the bands are as wide as
     # nx + ny + 1, i.e. the widest wavefront classes and the scan kernel.
-    d, cand = _dataset(60, 10, 7, genome_markers=4000, n50=6000, min_bases=4000)
-    rec, res = _compare(ctx, d, cand[:150], alignMethod=1, k=10, maxSkip=30, maxDrift=30, maxTrim=30,
-                        minAlignedMarkerCount=50, minAlignedFraction=0.3)
-    assert len(rec) > 10 and res.tooWideCount == 0
+    d, cand = candidate_set(60, 10, 7, genome_markers=4000, n50=6000, min_bases=4000)
+    rec = compare_alignments(ctx, d, cand[:150], alignMethod=1, k=10, maxSkip=30, maxDrift=30, maxTrim=30,
+                             minAlignedMarkerCount=50, minAlignedFraction=0.3)[0]
+    assert len(rec) > 10
 
 
 def test_alignment_properties(ctx):
     # Size-independent properties of the stored alignments: ordinals strictly increasing, codec round trip.
     from shasta_b200 import capi
-    d, cand = _dataset(200, 10, 33)
+    d, cand = candidate_set(200, 10, 33)
     ctx.set_markers(d["toc"], d["data"], d["flags"])
     rec, ctoc, cdata, _ = capi.compute_alignments(ctx, cand[:800], capi.make_align_options(k=10, minAlignedMarkerCount=50))
     assert len(rec)
@@ -112,20 +78,20 @@ def test_alignment_properties(ctx):
 def test_method4_default_cells(ctx):
     # Align4 (north_star's method): deltaX 200, deltaY 10, minEntryCountPerCell 10, maxDistanceFromBoundary 100
     # (src/AssemblerOptions.cpp:471-489); May2022-style filter values.
-    d, cand = _dataset(300, 10, 5)
-    rec, res = _compare(ctx, d, cand[:1200], alignMethod=4, k=10, maxSkip=100, maxDrift=100, maxTrim=100,
-                        minAlignedMarkerCount=10, minAlignedFraction=0.1, maxBand=1000)
+    d, cand = candidate_set(300, 10, 5)
+    rec, _, _, res = compare_alignments(ctx, d, cand[:1200], alignMethod=4, k=10, maxSkip=100, maxDrift=100, maxTrim=100,
+                                        minAlignedMarkerCount=10, minAlignedFraction=0.1, maxBand=1000)
     assert len(rec) > 100 and res.dpCells > 0
 
 
 def test_method4_small_cells_strict_and_containments(ctx):
-    d, cand = _dataset(250, 14, 9)
-    _compare(ctx, d, cand[:800], alignMethod=4, k=14, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=60,
-             minAlignedFraction=0.4, align4DeltaX=100, align4DeltaY=5, align4MinEntryCountPerCell=4,
-             align4MaxDistanceFromBoundary=50, maxBand=300)
-    _compare(ctx, d, cand[:800], alignMethod=4, k=14, maxSkip=100, maxDrift=100, maxTrim=100, minAlignedMarkerCount=10,
-             minAlignedFraction=0.1, align4DeltaX=50, align4DeltaY=20, align4MinEntryCountPerCell=1,
-             align4MaxDistanceFromBoundary=1000, maxBand=100, suppressContainments=1)
+    d, cand = candidate_set(250, 14, 9)
+    compare_alignments(ctx, d, cand[:800], alignMethod=4, k=14, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=60,
+                       minAlignedFraction=0.4, align4DeltaX=100, align4DeltaY=5, align4MinEntryCountPerCell=4,
+                       align4MaxDistanceFromBoundary=50, maxBand=300)
+    compare_alignments(ctx, d, cand[:800], alignMethod=4, k=14, maxSkip=100, maxDrift=100, maxTrim=100, minAlignedMarkerCount=10,
+                       minAlignedFraction=0.1, align4DeltaX=50, align4DeltaY=20, align4MinEntryCountPerCell=1,
+                       align4MaxDistanceFromBoundary=1000, maxBand=100, suppressContainments=1)
 
 
 @pytest.mark.parametrize("smem_cells", ["1", "6"])
@@ -133,29 +99,29 @@ def test_method4_front_end_global_path(ctx, monkeypatch, smem_cells):
     """The Align4 front end keeps a candidate's existing cells in shared memory when they fit; candidates with more
     cells take the global-memory path. A tiny limit sends (nearly) every candidate through that path."""
     monkeypatch.setenv("SHB_ALIGN4_SMEM_CELLS", smem_cells)
-    d, cand = _dataset(250, 14, 9)
-    _compare(ctx, d, cand[:600], alignMethod=4, k=14, maxSkip=100, maxDrift=100, maxTrim=100, minAlignedMarkerCount=10,
-             minAlignedFraction=0.1, align4DeltaX=50, align4DeltaY=20, align4MinEntryCountPerCell=1,
-             align4MaxDistanceFromBoundary=1000, maxBand=100)
-    _compare(ctx, d, cand[:600], alignMethod=4, k=14, maxSkip=100, maxDrift=100, maxTrim=100,
-             minAlignedMarkerCount=10, minAlignedFraction=0.1, maxBand=1000)
+    d, cand = candidate_set(250, 14, 9)
+    compare_alignments(ctx, d, cand[:600], alignMethod=4, k=14, maxSkip=100, maxDrift=100, maxTrim=100, minAlignedMarkerCount=10,
+                       minAlignedFraction=0.1, align4DeltaX=50, align4DeltaY=20, align4MinEntryCountPerCell=1,
+                       align4MaxDistanceFromBoundary=1000, maxBand=100)
+    compare_alignments(ctx, d, cand[:600], alignMethod=4, k=14, maxSkip=100, maxDrift=100, maxTrim=100,
+                       minAlignedMarkerCount=10, minAlignedFraction=0.1, maxBand=1000)
 
 
 def test_method4_random_pairs(ctx):
-    d, _ = _dataset(120, 10, 21)
+    d, _ = candidate_set(120, 10, 21)
     rng = np.random.default_rng(5)
     a = rng.integers(0, 119, 500)
     b = rng.integers(0, 119, 500)
     lo, hi = np.minimum(a, b), np.maximum(a, b)
     ok = lo < hi
     cand = np.stack([lo[ok], hi[ok], rng.integers(0, 2, ok.sum())], 1).astype(np.uint32)
-    _compare(ctx, d, cand, alignMethod=4, k=10, maxSkip=100, maxDrift=100, maxTrim=1000, minAlignedMarkerCount=5,
-             minAlignedFraction=0.05, align4MinEntryCountPerCell=2, maxBand=2000)
+    compare_alignments(ctx, d, cand, alignMethod=4, k=10, maxSkip=100, maxDrift=100, maxTrim=1000, minAlignedMarkerCount=5,
+                       minAlignedFraction=0.05, align4MinEntryCountPerCell=2, maxBand=2000)
 
 
 def test_alignment_table(ctx):
     from shasta_b200 import capi
-    d, cand = _dataset(200, 10, 33)
+    d, cand = candidate_set(200, 10, 33)
     ctx.set_markers(d["toc"], d["data"], d["flags"])
     rec, _, _, _ = capi.compute_alignments(ctx, cand[:900], capi.make_align_options(k=10, minAlignedMarkerCount=50))
     toc, table = capi.compute_alignment_table(ctx, rec, 200)
@@ -170,7 +136,7 @@ def test_alignment_table(ctx):
 
 def test_candidate_table(ctx):
     from shasta_b200 import capi
-    d, cand = _dataset(200, 10, 33)
+    d, cand = candidate_set(200, 10, 33)
     toc, table = capi.compute_candidate_table(ctx, cand, 200)
     otoc, otable = B.oracle_compute_candidate_table(cand, 200)
     assert len(cand) > 500
@@ -186,19 +152,16 @@ def test_candidate_table(ctx):
 def test_all_band_classes(ctx, band_extend, max_band):
     # bandExtend widens the stage-2 band so that every kernel class is exercised: the register-resident wavefront kernel
     # with C = 2, 3, 4, 6, 8, 12, 16 sub-chunk widths, and the shared-memory scan kernel for bands wider than 1024.
-    d, cand = _dataset(150, 10, 45)
-    _compare(ctx, d, cand[:250], alignMethod=3, k=10, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=50,
-             minAlignedFraction=0.3, downsamplingFactor=0.1, bandExtend=band_extend, maxBand=max_band)
+    d, cand = candidate_set(150, 10, 45)
+    compare_alignments(ctx, d, cand[:250], alignMethod=3, k=10, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=50,
+                       minAlignedFraction=0.3, downsamplingFactor=0.1, bandExtend=band_extend, maxBand=max_band)
 
 
 def test_long_reads_wide_stage1(ctx):
     # Ultra-long-like reads: stage 1 runs on ~700 downsampled markers per read (band classes C = 12/16 and the scan kernel).
-    p = synth.SynthParams(reads=24, k=10, genome_markers=9000, n50_bases=90000, min_bases=60000, seed=3, sigma=0.2)
-    d = synth.generate(p)
-    lp = B.LowHashParams(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2, maxBucketSize=30, minFrequency=2)
-    cand, _, _ = B.oracle_lowhash0(d["toc"], d["data"], d["flags"], lp)
+    d, cand = candidate_set(24, 10, 3, genome_markers=9000, n50=90000, min_bases=60000, sigma=0.2)
     assert len(cand) > 20
-    _compare(ctx, d, cand[:60], alignMethod=3, k=10, maxSkip=100, maxDrift=100, maxTrim=100, minAlignedMarkerCount=10,
-             minAlignedFraction=0.1, downsamplingFactor=0.15, bandExtend=10, maxBand=1000)
-    _compare(ctx, d, cand[:60], alignMethod=4, k=10, maxSkip=100, maxDrift=100, maxTrim=100, minAlignedMarkerCount=10,
-             minAlignedFraction=0.1, maxBand=1000)
+    compare_alignments(ctx, d, cand[:60], alignMethod=3, k=10, maxSkip=100, maxDrift=100, maxTrim=100, minAlignedMarkerCount=10,
+                       minAlignedFraction=0.1, downsamplingFactor=0.15, bandExtend=10, maxBand=1000)
+    compare_alignments(ctx, d, cand[:60], alignMethod=4, k=10, maxSkip=100, maxDrift=100, maxTrim=100, minAlignedMarkerCount=10,
+                       minAlignedFraction=0.1, maxBand=1000)

@@ -32,11 +32,10 @@ for _path in (HERE, ROOT):                      # run as the per-policy subproce
     if _path not in sys.path:
         sys.path.insert(0, _path)
 
-import test_gpu_align_limits as AL  # noqa: E402
 from oracle import bindings as B  # noqa: E402
-from shasta_b200 import synth  # noqa: E402
+from support import (PERMISSIVE, K, Genome, assemble, candidate_set, downsampled, downsampling_hash,  # noqa: E402
+                     downsampling_threshold, expected_single_pair, oracle_options, row, single_pair_options)
 
-K = AL.K
 DEFAULT_POLICY = 7
 POLICY_DIR = os.path.join(ROOT, "shasta_b200", "lib", "dp_policy")
 # The shipped 6/-1/-1 and variants, then unusual but legal sets: every path ties (0/0/0), a mismatch scoring above a match
@@ -63,16 +62,13 @@ def scores(name):
 @functools.lru_cache(None)
 def k10_set():
     """The k = 10 synthetic reads with their LowHash candidates."""
-    d = synth.generate(synth.SynthParams(reads=150, k=K, genome_markers=12000, n50_bases=12000, min_bases=6000, seed=11))
-    lp = B.LowHashParams(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2, maxBucketSize=30, minFrequency=2)
-    cand, _, _ = B.oracle_lowhash0(d["toc"], d["data"], d["flags"], lp)
-    return d, cand
+    return candidate_set(150, K, 11, genome_markers=12000, n50=12000, min_bases=6000)
 
 
 def few_kmer_values(count, factor, seed, kept=True):
     """`count` k-mer ids that the downsampling at `factor` keeps (kept) or drops."""
     ids = np.random.default_rng(seed).integers(0, 1 << (2 * K), 256).astype(np.uint32)
-    keep = AL.downsampling_hash(ids, K) < np.uint32(int(factor * 4294967295.0))
+    keep = downsampling_hash(ids, K) < downsampling_threshold(factor)
     return ids[keep == kept][:count]
 
 
@@ -86,13 +82,13 @@ def tie_set():
     """Reads of 20 to 2 000 markers cut from a genome of eight k-mer ids (inserted markers are random), four of which the
     downsampling at TIE_FACTOR keeps: ties everywhere, in both stages of method 3. Every pair on the same strand, and a
     few on opposite strands."""
-    genome = AL.Genome(6000, seed=5, drop=0.04, ins=0.02)
+    genome = Genome(6000, seed=5, drop=0.04, ins=0.02)
     values = np.concatenate([few_kmer_values(4, TIE_FACTOR, 3), few_kmer_values(4, TIE_FACTOR, 3, kept=False)])
     genome.kmer = genome.rng.choice(values, len(genome.kmer)).astype(np.uint32)
     rows = [genome.read(s, L)[0] for s, L in zip(TIE_STARTS, TIE_LENGTHS)]
     n = len(rows)
     cand = [(i, j, 1) for i in range(n) for j in range(i + 1, n)] + [(i, i + 1, 0) for i in range(0, n - 1, 3)]
-    return AL.assemble(rows), np.array(cand, np.uint32)
+    return assemble(rows, K), np.array(cand, np.uint32)
 
 
 END_CELL_M = (1, 5, 20, 40, 75)        # ny = 7m: forward groups of 8, 8, 16, 32 lanes; 525 > 512 rows: the traced path
@@ -111,7 +107,7 @@ def end_cell_set():
     rows = []
     for m in END_CELL_M:
         rows += end_cell_rows(m, rng)
-    return AL.assemble(rows), np.array([(2 * i, 2 * i + 1, 1) for i in range(len(END_CELL_M))], np.uint32)
+    return assemble(rows, K), np.array([(2 * i, 2 * i + 1, 1) for i in range(len(END_CELL_M))], np.uint32)
 
 
 TIE_PAIRS = ((2, 5), (4, 9), (6, 8), (8, 9), (3, 4), (0, 2))
@@ -136,9 +132,9 @@ class Case(NamedTuple):
     oriented: bool = False
 
 
-M3_TIES = dict(AL.PERMISSIVE, alignMethod=3, downsamplingFactor=TIE_FACTOR, maxBand=2000)
+M3_TIES = dict(PERMISSIVE, alignMethod=3, downsamplingFactor=TIE_FACTOR, maxBand=2000)
 TIE_EXTENDS = (2, 10, 30, 100, 600)     # stage-2 bands on the 8-lane groups, the whole-warp classes and the scan kernel
-END_CELL_OPTS = dict(AL.PERMISSIVE, alignMethod=3, downsamplingFactor=1.0, bandExtend=2, maxBand=1000)
+END_CELL_OPTS = dict(PERMISSIVE, alignMethod=3, downsamplingFactor=1.0, bandExtend=2, maxBand=1000)
 
 
 def k10_candidates():
@@ -150,17 +146,17 @@ def cases():
     # Method 3 on the tie-rich reads: stage 1 on every forward class and on the traced path, stage 2 on every band class.
     out = [Case(f"m3_ties_e{e}", tie_set, dict(M3_TIES, bandExtend=e)) for e in TIE_EXTENDS]
     for s in SCORES:
-        out.append(Case(f"m1_ties_s{s}", tie_set, dict(AL.PERMISSIVE, alignMethod=1, **scores(s))))
+        out.append(Case(f"m1_ties_s{s}", tie_set, dict(PERMISSIVE, alignMethod=1, **scores(s))))
         if s != "6_1_1":
             out.append(Case(f"m3_ties_s{s}", tie_set, dict(M3_TIES, bandExtend=10, **scores(s))))
-    out.append(Case("m4_ties", tie_set, AL.single_pair_options(4)))
+    out.append(Case("m4_ties", tie_set, single_pair_options(4)))
     for s in ("6_1_1", "6_1_3"):
-        out.append(Case(f"m3_k10_s{s}", k10_candidates, dict(AL.PERMISSIVE, alignMethod=3, minAlignedMarkerCount=30,
+        out.append(Case(f"m3_k10_s{s}", k10_candidates, dict(PERMISSIVE, alignMethod=3, minAlignedMarkerCount=30,
                                                            minAlignedFraction=0.2, **scores(s))))
-    out.append(Case("m4_k10", k10_candidates, AL.single_pair_options(4)))
+    out.append(Case("m4_k10", k10_candidates, single_pair_options(4)))
     out.append(Case("m3_end_cell", end_cell_set, END_CELL_OPTS))
     for method in (1, 3, 4):
-        opts = dict(AL.single_pair_options(method), **(dict(downsamplingFactor=TIE_FACTOR) if method == 3 else {}))
+        opts = dict(single_pair_options(method), **(dict(downsamplingFactor=TIE_FACTOR) if method == 3 else {}))
         out.append(Case(f"oriented_m{method}", tie_pair_set, opts, oriented=True))
     return out
 
@@ -192,16 +188,12 @@ def run_device(lib_path, out_dir):
 
 
 # ---- the oracle side -------------------------------------------------------------------------------------------------
-def oracle_options(opts):
-    return B.make_align_options(**{k: v for k, v in opts.items() if k in B.ALIGN_DEFAULTS})
-
-
 def _oracle_case(case):
     d, work = case.data()
     if case.oriented:
         expected = []
         for o0, o1 in work:
-            exp = AL.expected_single_pair(AL.row(d, o0), AL.row(d, o1), case.opts)
+            exp = expected_single_pair(row(d, o0), row(d, o1), case.opts)
             expected.append(None if exp is None else (exp[0][3:16].copy(), exp[1]))
         return expected
     return B.oracle_compute_alignments(d["toc"], d["kmer"], work, oracle_options(case.opts), threads=8)[:3]
@@ -270,15 +262,9 @@ def test_policy_matches_oracle(policy, tmp_path):
 
 
 # ---- host checks -----------------------------------------------------------------------------------------------------
-def downsampled(row, factor):
-    """(k-mers, ordinals) that method 3's stage 1 keeps of a row."""
-    keep = np.flatnonzero(AL.downsampling_hash(row, K) < np.uint32(int(factor * 4294967295.0)))
-    return row[keep], keep.astype(np.int64)
-
-
 def candidate_rows(d, c):
     r0, r1, same = (int(x) for x in c)
-    return AL.row(d, 2 * r0), AL.row(d, 2 * r1 + (0 if same else 1))
+    return row(d, 2 * r0), row(d, 2 * r1 + (0 if same else 1))
 
 
 def band_class(W):
@@ -360,7 +346,7 @@ def test_cases_reach_their_paths():
         assert any(any((x is None) != (y is None) or (x is not None and not np.array_equal(x[1], y[1])) for x, y in zip(o, out[0]))
                    for o in out[1:]), m
     # tie-rich: eight k-mer ids make up all but the inserted markers, and the downsampling keeps four of them
-    strand0 = np.concatenate([AL.row(d, 2 * r) for r in range(len(d["flags"]))])
+    strand0 = np.concatenate([row(d, 2 * r) for r in range(len(d["flags"]))])
     values, counts = np.unique(strand0, return_counts=True)
     top = values[np.argsort(counts)[-8:]]
     assert np.isin(strand0, top).mean() > 0.95 and len(downsampled(top, TIE_FACTOR)[0]) == 4

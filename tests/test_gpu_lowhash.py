@@ -3,26 +3,17 @@ C ABI, against the reference's golden vectors and against the CPU oracle on the 
 Bar: bit-exact candidates (order included) and ReadLowHashStatistics."""
 import json
 import os
-import sys
 
 import numpy as np
 import pytest
 
 from oracle import bindings as B
 from shasta_b200 import synth
+from support import LOWHASH, TILE, ctx, feature_hashes, hash_threshold  # noqa: F401
 
-sys.path.insert(0, os.path.join(os.path.dirname(__file__), "golden"))
-import make_golden as MG  # noqa: E402
+import make_golden as MG
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from shasta_b200 import capi
-    c = capi.Context(0)
-    yield c
-    c.close()
 
 
 def _params(capi, params, **extra):
@@ -109,18 +100,17 @@ def test_tinytest_pin_through_host_call(ctx, golden_dir):
 @pytest.mark.parametrize("m", [1, 2, 3, 6, 7, 8, 9, 12, 13, 16, 31, 32])
 def test_feature_lengths_against_oracle(ctx, m):
     from shasta_b200 import capi
-    import test_gpu_lowhash_paths as P
     d = synth.generate(synth.SynthParams(reads=120, k=10, genome_markers=15000, n50_bases=12000, min_bases=6000, seed=40 + m))
     kw = dict(m=m, hashFraction=0.02, minHashIterationCount=5, minBucketSize=0, maxBucketSize=20, minFrequency=1)
     if m > 8:
         # Generic kernel (m > 8): some low hash of the launch starts at the last position of a full tile, so that its
         # feature reads m - 1 words of the halo that follows the tile (at m = 32, up to its last word).
         M = int(d["toc"][-1])
-        local = np.arange(P.TILE - m + 1, P.TILE)
-        positions = (np.arange(1, M // P.TILE)[:, None] * P.TILE + local[None, :] - P.TILE).ravel()
-        h = P.feature_hashes(d["kmer"], m, [37 * s for s in range(5)], positions=positions)
-        halo = (h < np.uint64(P.hash_threshold(0.02))).any(0)
-        assert (positions[halo] % P.TILE == P.TILE - 1).any()
+        local = np.arange(TILE - m + 1, TILE)
+        positions = (np.arange(1, M // TILE)[:, None] * TILE + local[None, :] - TILE).ravel()
+        h = feature_hashes(d["kmer"], m, [37 * s for s in range(5)], positions=positions)
+        halo = (h < np.uint64(hash_threshold(0.02))).any(0)
+        assert (positions[halo] % TILE == TILE - 1).any()
     ctx.set_markers(d["toc"], d["data"], d["flags"])
     cand, stats, _, _ = ctx.lowhash0(capi.make_lowhash_params(**kw))
     oc, os_, _ = B.oracle_lowhash0(d["toc"], d["data"], d["flags"], B.LowHashParams(**kw))
@@ -233,10 +223,9 @@ def test_device_generator_matches_numpy(ctx):
     assert np.array_equal(dm.data7_to_host(), d["data"])
     assert np.array_equal(dm.flags, d["flags"])
     # Device-resident path gives the same candidates as the host-upload path.
-    kw = dict(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2, maxBucketSize=30, minFrequency=2)
     ctx.set_markers_device(dm.toc, dm.kmer_ptr, dm.flags, keepalive=dm)
-    c1, s1, _, _ = ctx.lowhash0(capi.make_lowhash_params(**kw))
+    c1, s1, _, _ = ctx.lowhash0(capi.make_lowhash_params(**LOWHASH))
     ctx.set_markers(d["toc"], d["data"], d["flags"])
-    c2, s2, _, _ = ctx.lowhash0(capi.make_lowhash_params(**kw))
+    c2, s2, _, _ = ctx.lowhash0(capi.make_lowhash_params(**LOWHASH))
     assert np.array_equal(c1, c2) and np.array_equal(s1, s2) and len(c1) > 0
     dm.free()

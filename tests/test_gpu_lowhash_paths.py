@@ -6,75 +6,27 @@ Bar: bit-exact candidates (order included) and ReadLowHashStatistics against the
 Every test first checks on the host that its input reaches the path it is for (queued hits per tile, reads per tile, low
 hashes per iteration), with a numpy MurmurHash64A that is itself checked against the oracle's."""
 import os
-import sys
 
 import numpy as np
 import pytest
 
 from oracle import bindings as B
 from shasta_b200 import synth
+from support import LOWHASH, TILE, assemble, ctx, feature_hashes, hash_threshold, strand0_rows  # noqa: F401
 
-sys.path.insert(0, os.path.join(os.path.dirname(__file__), "golden"))
-import make_golden as MG  # noqa: E402
+import make_golden as MG
 
 pytestmark = pytest.mark.gpu
 
 U64 = np.uint64
-MURMUR_M = U64(0xc6a4a7935bd1e995)
-TILE = 2048                     # kSweepTile (csrc/lowhash_kernels.cuh)
 TILE_READS = 32                 # kSweepTileReads
 QUEUE_MIN, QUEUE_MAX = 256, 6144
 UNROLLED_GROUPS = (16, 10, 8, 4, 2, 1)
 
-NANOPORE = dict(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2, maxBucketSize=30, minFrequency=2)
 HIFI = dict(m=4, hashFraction=0.05, minHashIterationCount=20, minBucketSize=10, maxBucketSize=60, minFrequency=3)
 
 
-@pytest.fixture(scope="module")
-def ctx():
-    from shasta_b200 import capi
-    c = capi.Context(0)
-    yield c
-    c.close()
-
-
 # ---- host model of the sweep ---------------------------------------------------------------------------------------
-def feature_hashes(kmer, m, seeds, positions=None):
-    """MurmurHash64A of the 4*m bytes of k-mer ids starting at each position (all p with p + m <= len(kmer) by default),
-    for every seed: uint64[len(seeds), len(positions)]."""
-    kmer = np.asarray(kmer, np.uint32)
-    if positions is None:
-        positions = np.arange(max(len(kmer) - m + 1, 0), dtype=np.int64)
-    positions = np.asarray(positions, np.int64)
-    with np.errstate(over="ignore"):
-        mixed = []
-        for b in range(m // 2):
-            k = kmer[positions + 2 * b].astype(U64) | (kmer[positions + 2 * b + 1].astype(U64) << U64(32))
-            k *= MURMUR_M
-            k ^= k >> U64(47)
-            k *= MURMUR_M
-            mixed.append(k)
-        tail = kmer[positions + m - 1].astype(U64) if m & 1 else None
-        out = np.empty((len(seeds), len(positions)), U64)
-        for i, seed in enumerate(seeds):
-            h = np.full(len(positions), U64(seed) ^ (U64(4 * m) * MURMUR_M), U64)
-            for k in mixed:
-                h ^= k
-                h *= MURMUR_M
-            if tail is not None:
-                h ^= tail
-                h *= MURMUR_M
-            h ^= h >> U64(47)
-            h *= MURMUR_M
-            h ^= h >> U64(47)
-            out[i] = h
-    return out
-
-
-def hash_threshold(hash_fraction):
-    return int(hash_fraction * 18446744073709551616.0)         # uint64_t(hashFraction * double(UINT64_MAX))
-
-
 def sweep_groups(params):
     """Iterations fused into one sweep launch, in order (lowhash0 in csrc/lowhash.cu); None when the candidate count decides
     the number of iterations (groups of one)."""
@@ -112,26 +64,6 @@ def valid_feature_mask(toc, flags, m):
     row = np.repeat(np.arange(len(toc) - 1), np.diff(toc))
     ok = (np.arange(M) + m <= toc[row + 1]) & (np.asarray(flags)[row >> 1] & 1 == 0)
     return ok[:max(M - m + 1, 0)]
-
-
-def assemble(rows0, k, flags):
-    """Marker set from the strand-0 rows; every strand-1 row is the reverse complement of its strand-0 row."""
-    lengths = np.array([len(r) for r in rows0], np.int64)
-    toc = np.zeros(2 * len(rows0) + 1, np.uint64)
-    toc[1:] = np.cumsum(np.repeat(lengths, 2)).astype(np.uint64)
-    parts = []
-    for r in rows0:
-        r = np.asarray(r, np.uint32)
-        parts.append(r)
-        parts.append(synth.reverse_complement_kmer(r[::-1], k))
-    kmer = np.concatenate(parts).astype(np.uint32) if parts else np.zeros(0, np.uint32)
-    pos = (np.arange(len(kmer)) % (1 << 24)).astype(np.uint32)
-    return dict(toc=toc, kmer=kmer, data=synth.pack_markers(kmer, pos), flags=np.asarray(flags, np.uint8))
-
-
-def strand0_rows(d):
-    toc = d["toc"].astype(np.int64)
-    return [d["kmer"][toc[2 * r]:toc[2 * r + 1]].copy() for r in range(len(d["flags"]))]
 
 
 def compare_with_oracle(ctx, d, params):
@@ -186,7 +118,7 @@ def tandem_repeat_dataset():
 @pytest.mark.parametrize("aggregate", ["0", "1"])
 @pytest.mark.parametrize("config", ["nanopore", "hifi"])
 def test_tandem_repeats_overflow_the_sweep_queue(ctx, monkeypatch, aggregate, config):
-    params = NANOPORE if config == "nanopore" else HIFI
+    params = LOWHASH if config == "nanopore" else HIFI
     d, in_repeat = tandem_repeat_dataset()
     overflowing, ordinary_spill = 0, 0
     first = 0
@@ -303,7 +235,7 @@ def test_tiles_with_many_short_reads(ctx):
 
 # ---- A. slab regrowth ----------------------------------------------------------------------------------------------
 def test_slab_regrowth(ctx):
-    params = dict(NANOPORE)
+    params = dict(LOWHASH)
     k, m, hf = 10, params["m"], params["hashFraction"]
     base = synth.generate(synth.SynthParams(reads=30, k=k, genome_markers=20000, n50_bases=12000, min_bases=6000, seed=13))
     # A k-mer whose feature (the k-mer m times) is a low hash in some iteration of the (only) group.
@@ -328,7 +260,7 @@ def test_misaligned_kmer_ids(ctx, offset):
     import torch
     from shasta_b200 import capi
     d = synth.generate(synth.SynthParams(reads=200, k=10, genome_markers=25000, n50_bases=12000, min_bases=6000, seed=8))
-    params = NANOPORE
+    params = LOWHASH
     M = int(d["toc"][-1])
     buf = torch.zeros(M + 8, dtype=torch.int32, device="cuda")
     buf[offset:offset + M] = torch.from_numpy(d["kmer"].view(np.int32)).cuda()

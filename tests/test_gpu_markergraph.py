@@ -2,35 +2,23 @@
 restatement (oracle/markergraph_oracle.c), which tests/test_oracle_markergraph.py pins to the reference's own components.
 Both number vertices by their first marker, so the device's outputs must equal the oracle's exactly."""
 import os
-import sys
 
 import numpy as np
 import pytest
 
 from oracle import markergraph_bindings as MB
+from support import PaddedSet, ctx, device_read_graph, need_memory, pack_ordinal_markers  # noqa: F401
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-from markergraph_inputs import PARAMS, _finish, cases  # noqa: E402
+from markergraph_inputs import PARAMS, _finish, cases
 
 pytestmark = pytest.mark.gpu
 CASES = cases()
 INV40 = (1 << 40) - 1
 
 
-@pytest.fixture(scope="module")
-def ctx():
-    from shasta_b200 import capi
-    c = capi.Context(0)
-    yield c
-    c.close()
-
-
 def _upload(ctx, d):
-    from shasta_b200 import synth
     toc = d["toc"]
-    pos = np.concatenate([np.arange(toc[i + 1] - toc[i], dtype=np.uint32) for i in range(len(toc) - 1)] or [np.zeros(0, np.uint32)])
-    ctx.set_markers(toc, synth.pack_markers(np.asarray(d["kmer"], np.uint32), pos), np.zeros((len(toc) - 1) // 2, np.uint8))
+    ctx.set_markers(toc, pack_ordinal_markers(toc, d["kmer"]), np.zeros((len(toc) - 1) // 2, np.uint8))
 
 
 def _device(ctx, d, **params):
@@ -216,26 +204,10 @@ def test_large_sets(ctx):
 
 
 def _pipeline(method):
-    from shasta_b200 import capi, synth
-    d = synth.generate(synth.SynthParams(reads=400, k=10, genome_markers=40000, n50_bases=12000, min_bases=6000, seed=9))
-    c = capi.Context(0)
-    try:
-        c.set_markers(d["toc"], d["data"], d["flags"])
-        cand, _, _, _ = c.lowhash0(capi.make_lowhash_params(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2,
-                                                           maxBucketSize=30, minFrequency=2))
-        akw = dict(alignMethod=3, k=10, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=50, minAlignedFraction=0.3,
-                   downsamplingFactor=0.1, bandExtend=10, maxBand=1000)
-        rec, ctoc, cdata, _ = capi.compute_alignments(c, cand, capi.make_align_options(**akw))
-        rec = np.array(rec, np.uint32)
-        if method == 0:
-            _, edges, _, _ = capi.create_read_graph(c, rec, 400, 6)
-        else:
-            _, _, edges, _, _ = capi.create_read_graph2(c, rec, 400, 6, 0.015, 0.12, 0.12, 0.12, 0.015)
+    with device_read_graph(method) as (_, d, _, ctoc, cdata, (edges, _, _)):
         flags = np.array(d["flags"], np.uint8)
         flags[::37] |= 2                                                    # a few chimeric reads
-        return dict(toc=d["toc"], kmer=d["kmer"], edges=np.array(edges), ctoc=np.array(ctoc), cdata=np.array(cdata), flags=flags)
-    finally:
-        c.close()
+        return dict(toc=d["toc"], kmer=d["kmer"], edges=edges, ctoc=ctoc, cdata=cdata, flags=flags)
 
 
 @pytest.mark.parametrize("method", [0, 2])
@@ -257,10 +229,8 @@ def test_facade_files(tmp_path, monkeypatch):
     prefix = str(tmp_path / "Data") + "/"
     os.makedirs(prefix)
     R = (len(d["toc"]) - 1) // 2
-    from shasta_b200 import synth
-    pos = np.concatenate([np.arange(d["toc"][i + 1] - d["toc"][i], dtype=np.uint32) for i in range(2 * R)])
     A.mm_write_vector(prefix + "Markers.toc", d["toc"])
-    A.mm_write_vector(prefix + "Markers.data", synth.pack_markers(d["kmer"], pos), object_size=7)
+    A.mm_write_vector(prefix + "Markers.data", pack_ordinal_markers(d["toc"], d["kmer"]), object_size=7)
     A.mm_write_vector(prefix + "ReadFlags", np.zeros(R, np.uint8))
     A.mm_write_vector(prefix + "ReadGraphEdges", d["edges"], object_size=16)
     A.mm_write_vector_of_vectors(prefix + "CompressedAlignments", d["ctoc"], d["cdata"], data_object_size=1)
@@ -294,12 +264,11 @@ def test_facade_files(tmp_path, monkeypatch):
 def test_marker_ids_past_2_32(ctx):
     """A read graph on real reads placed after 2^32 filler markers (filler reads are singletons, dropped by minCoverage 2)."""
     import torch
-    import test_gpu_large_offsets as LO
     from shasta_b200 import capi
-    LO.need_memory(64)
+    need_memory(64)
     d = _pipeline(0)
     real = dict(toc=d["toc"], kmer=d["kmer"], flags=np.zeros((len(d["toc"]) - 1) // 2, np.uint8))
-    padded = LO.PaddedSet(real, 10, 12345)
+    padded = PaddedSet(real, 10, 12345)
     padded.reals(5)
     padded.fill_to(((1 << 32) + 1000) & ~1)
     padded.reals(len(real["flags"]) - 5)

@@ -2,35 +2,22 @@
 restatement (oracle/markergraph_edges_oracle.c), which tests/test_oracle_markergraph_edges.py pins to the reference's own
 code. Both give the reference's one-thread output, so the device's outputs must equal the restatement's exactly."""
 import os
-import sys
 
 import numpy as np
 import pytest
 
 from oracle import markergraph_edges_bindings as EB
+from support import PaddedSet, ctx, device_read_graph, need_memory, pack_ordinal_markers  # noqa: F401
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-from markergraph_edges_inputs import large_vertex_case, vertex_cases  # noqa: E402
-from reference_outputs import recorded  # noqa: E402
+from markergraph_edges_inputs import drop_interval, large_vertex_case, parallel_edge, rc_failure_inputs, vertex_cases
+from reference_outputs import recorded, shrink
 
 pytestmark = pytest.mark.gpu
 CASES = vertex_cases()
 
 
-@pytest.fixture(scope="module")
-def ctx():
-    from shasta_b200 import capi
-    c = capi.Context(0)
-    yield c
-    c.close()
-
-
 def _upload(ctx, toc):
-    from shasta_b200 import synth
-    M = int(toc[-1])
-    pos = np.concatenate([np.arange(toc[i + 1] - toc[i], dtype=np.uint32) for i in range(len(toc) - 1)] or [np.zeros(0, np.uint32)])
-    ctx.set_markers(toc, synth.pack_markers(np.zeros(M, np.uint32), pos), np.zeros((len(toc) - 1) // 2, np.uint8))
+    ctx.set_markers(toc, pack_ordinal_markers(toc, np.zeros(int(toc[-1]), np.uint32)), np.zeros((len(toc) - 1) // 2, np.uint8))
 
 
 def _device(ctx, d):
@@ -67,12 +54,6 @@ def _check(ctx, d, rc_too=True):
     return out, res, rc
 
 
-def _shrink(a):
-    import hashlib
-    a = np.ascontiguousarray(a)
-    return np.frombuffer(hashlib.sha256(a.tobytes()).digest(), np.uint8) if a.size > 4096 else a
-
-
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_cases_against_oracle_and_reference(ctx, name):
     d = CASES[name]
@@ -83,9 +64,9 @@ def test_cases_against_oracle_and_reference(ctx, name):
     got = dict(fields=EB.named_fields(out["edges"]), itoc=out["intervalsToc"], idata=out["intervalsData"], stoc=out["bySourceToc"],
                sdata=EB.rows_from_uint40(out["bySourceData"]), ttoc=out["byTargetToc"], tdata=EB.rows_from_uint40(out["byTargetData"]))
     for k, v in got.items():
-        assert np.array_equal(_shrink(v).reshape(-1), np.asarray(ref[f"one/{k}"]).reshape(-1)), k
+        assert np.array_equal(shrink(v, 4096).reshape(-1), np.asarray(ref[f"one/{k}"]).reshape(-1)), k
     if rc is not None:
-        assert np.array_equal(_shrink(rc).reshape(-1), np.asarray(ref["one/rc"]).reshape(-1))
+        assert np.array_equal(shrink(rc, 4096).reshape(-1), np.asarray(ref["one/rc"]).reshape(-1))
 
 
 def test_byte_identical_runs(ctx):
@@ -121,29 +102,16 @@ def test_large_vertices(ctx):
 def _pipeline():
     """LowHash0 -> computeAlignments -> createReadGraph2 -> flagCrossStrandReadGraphEdges1 -> flagChimericReads -> vertices
     -> rc vertices on the device."""
-    from shasta_b200 import capi, synth
-    d = synth.generate(synth.SynthParams(reads=400, k=10, genome_markers=40000, n50_bases=12000, min_bases=6000, seed=9))
-    c = capi.Context(0)
-    try:
-        c.set_markers(d["toc"], d["data"], d["flags"])
-        cand, _, _, _ = c.lowhash0(capi.make_lowhash_params(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2,
-                                                           maxBucketSize=30, minFrequency=2))
-        akw = dict(alignMethod=3, k=10, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=50, minAlignedFraction=0.3,
-                   downsamplingFactor=0.1, bandExtend=10, maxBand=1000)
-        rec, ctoc, cdata, _ = capi.compute_alignments(c, cand, capi.make_align_options(**akw))
-        rec = np.array(rec, np.uint32)
-        _, keep, edges, ctoc_g, cdata_g = capi.create_read_graph2(c, rec, 400, 6, 0.015, 0.12, 0.12, 0.12, 0.015)
-        edges, ctoc_g, cdata_g = np.array(edges), np.array(ctoc_g), np.array(cdata_g)
+    from shasta_b200 import capi
+    with device_read_graph(2) as (c, d, rec, ctoc, cdata, (edges, ctoc_g, cdata_g)):
         capi.flag_cross_strand_read_graph_edges1(c, 6, edges, ctoc_g, cdata_g, rec)
         flags = np.array(d["flags"], np.uint8)
         capi.flag_chimeric_reads(c, 2, edges, ctoc_g, cdata_g, flags, rec)
         table, vtoc, vdata, _, res = capi.create_marker_graph_vertices(c, capi.make_marker_graph_params(minCoverage=2), edges,
-                                                                       np.array(ctoc), np.array(cdata), flags)
+                                                                       ctoc, cdata, flags)
         rc = capi.find_marker_graph_reverse_complement_vertices(c, table, vtoc, vdata)
         return dict(toc=d["toc"], table=capi.uint40_to_uint64(table), vtoc=capi.uint40_to_uint64(vtoc), vdata=np.array(vdata),
                     rc=np.array(rc)), d
-    finally:
-        c.close()
 
 
 def test_on_the_device_pipeline(ctx):
@@ -184,7 +152,6 @@ def test_invalid_inputs(ctx):
 
 def test_rc_failures(ctx):
     """The reference's two messages and its assertion, each as the restatement gives it; then a call that succeeds."""
-    import test_oracle_markergraph_edges as T
     from shasta_b200 import capi
     d = CASES["genome/cov2"]
     _upload(ctx, d["toc"])
@@ -193,7 +160,7 @@ def test_rc_failures(ctx):
         return capi.find_marker_graph_reverse_complement_edges(ctx, d["rc"], s["edges"], s["intervalsToc"], s["intervalsData"],
                                                                s["bySourceToc"], capi.uint64_to_uint40(s["bySourceData"]))
 
-    for name, _, s in T.rc_failure_inputs():
+    for name, _, s in rc_failure_inputs(d):
         msg, rc = EB.oracle_find_rc_edges(d["toc"], d["rc"], s)
         assert rc is None
         with pytest.raises(capi.ShastaB200Error) as e:
@@ -220,13 +187,12 @@ def test_rc_failures(ctx):
 
 def test_parallel_edges_first_match_in_stored_order(ctx):
     """Parallel edges whose intervals differ: the first match in stored row order, as the reference picks it."""
-    import test_oracle_markergraph_edges as T
     from shasta_b200 import capi
     d = CASES["genome/cov2"]
     _upload(ctx, d["toc"])
     o = EB.oracle_create_marker_graph_edges(d["toc"], d["table"], d["vtoc"], d["vdata"])
     cov = np.diff(o["intervalsToc"].astype(np.int64))
-    s = T._drop_interval(T._parallel(o, int(np.nonzero(cov >= 2)[0][3])), len(o["edges"]))    # the copy loses an interval
+    s = drop_interval(parallel_edge(o, int(np.nonzero(cov >= 2)[0][3])), len(o["edges"]))    # the copy loses an interval
     msg, orc = EB.oracle_find_rc_edges(d["toc"], d["rc"], s)
     rc = None
     try:
@@ -259,16 +225,15 @@ def test_sharded_context_is_refused(ctx):
 def test_facade_files(tmp_path, monkeypatch):
     """Assembler.createMarkerGraphEdges and findMarkerGraphReverseComplementEdges write files the reference's MemoryMapped
     code opens, with the restatement's contents."""
-    from shasta_b200 import assembler as A, capi, synth
+    from shasta_b200 import assembler as A, capi
     d = CASES["deep/strand1"]
     monkeypatch.chdir(tmp_path)
     prefix = str(tmp_path / "Data") + "/"
     os.makedirs(prefix)
     toc = d["toc"]
     M, R = int(toc[-1]), (len(toc) - 1) // 2
-    pos = np.concatenate([np.arange(toc[i + 1] - toc[i], dtype=np.uint32) for i in range(2 * R)])
     A.mm_write_vector(prefix + "Markers.toc", toc)
-    A.mm_write_vector(prefix + "Markers.data", synth.pack_markers(np.zeros(M, np.uint32), pos), object_size=7)
+    A.mm_write_vector(prefix + "Markers.data", pack_ordinal_markers(toc, np.zeros(M, np.uint32)), object_size=7)
     A.mm_write_vector(prefix + "ReadFlags", np.zeros(R, np.uint8))
     A.mm_write_vector(prefix + "MarkerGraphVertexTable", capi.uint64_to_uint40(d["table"]), object_size=5)
     A.mm_write_vector(prefix + "MarkerGraphVertices.toc", capi.uint64_to_uint40(d["vtoc"]), object_size=5)
@@ -296,12 +261,11 @@ def test_facade_files(tmp_path, monkeypatch):
 def test_marker_ids_past_2_32(ctx):
     """Vertices on reads placed after 2^32 filler markers that carry no vertex."""
     import torch
-    import test_gpu_large_offsets as LO
     from shasta_b200 import capi
-    LO.need_memory(48)
+    need_memory(48)
     d = CASES["genome/cov2"]
     real = dict(toc=d["toc"], kmer=np.zeros(int(d["toc"][-1]), np.uint32), flags=np.zeros((len(d["toc"]) - 1) // 2, np.uint8))
-    padded = LO.PaddedSet(real, 10, 12345)
+    padded = PaddedSet(real, 10, 12345)
     padded.reals(5)
     padded.fill_to(((1 << 32) + 1000) & ~1)
     padded.reals(len(real["flags"]) - 5)

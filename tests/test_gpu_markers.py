@@ -11,17 +11,10 @@ import numpy as np
 import pytest
 
 from oracle import bindings as B
+from support import ctx, reference_markers  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from shasta_b200 import capi
-    c = capi.Context(0)
-    yield c
-    c.close()
 
 
 def _golden():
@@ -52,7 +45,6 @@ def test_tinytest_markers_bit_for_bit(ctx):
 
 @pytest.mark.parametrize("k", [6, 10, 14])
 def test_synthetic_fasta_against_live_reference(ctx, tmp_path, k):
-    from test_oracle_markers import reference_markers
     g = reference_markers(tmp_path, 60, k, k)
     ids = g["marker_kmers"].astype(np.uint64)
     bitmap = np.zeros(max(1, 4 ** k // 32), np.uint32)

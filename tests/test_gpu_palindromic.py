@@ -1,37 +1,22 @@
 """flagPalindromicReads on the GPU (csrc/palindromic.cu, shb_flag_palindromic_reads) against the C restatement
 (oracle/palindromic_oracle.c), which tests/test_oracle_palindromic.py pins to the reference build."""
 import os
-import sys
 
 import numpy as np
 import pytest
 
 from oracle import palindromic_bindings as B
+from support import LOWHASH, ctx, pack_ordinal_markers  # noqa: F401
+
+from palindromic_inputs import cases, killer_case, oriented, palindrome, reverse_complement, rows_to_case
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-from palindromic_inputs import cases, killer_case, oriented, palindrome, reverse_complement, rows_to_case  # noqa: E402
-
 CASES = cases()
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from shasta_b200 import capi
-    c = capi.Context(0)
-    yield c
-    c.close()
-
-
-def _data7(toc, ids):
-    from shasta_b200 import synth
-    pos = np.concatenate([np.arange(toc[i + 1] - toc[i], dtype=np.uint32) for i in range(len(toc) - 1)] or [np.zeros(0, np.uint32)])
-    return synth.pack_markers(np.asarray(ids, np.uint32), pos)
 
 
 def _upload(ctx, toc, ids, flags=None):
     R = (len(toc) - 1) // 2
-    ctx.set_markers(toc, _data7(toc, ids), np.zeros(R, np.uint8) if flags is None else flags)
+    ctx.set_markers(toc, pack_ordinal_markers(toc, ids), np.zeros(R, np.uint8) if flags is None else flags)
 
 
 def _params(p):
@@ -117,8 +102,7 @@ def test_lowhash0_sees_new_flags(ctx):
     o = B.oracle_flag_palindromic(toc, kmer, **params)
     assert o["flags"].sum() >= R // 50
     data7 = synth.pack_markers(kmer, d["pos"])
-    kw = dict(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2, maxBucketSize=30, minFrequency=2)
-    lp = capi.make_lowhash_params(**kw)
+    lp = capi.make_lowhash_params(**LOWHASH)
     ctx.set_markers(toc, data7, flags0)
     flags = flags0.copy()
     capi.flag_palindromic_reads(ctx, _params(params), read_flags=flags)
@@ -153,7 +137,7 @@ def test_sharded_context_refused(ctx):
     R = (len(toc) - 1) // 2
     half = R // 2
     local = toc[:2 * half + 1]
-    ctx.set_markers(local, _data7(local, ids[:int(local[-1])]), np.zeros(R, np.uint8), read_begin=0, read_end=half,
+    ctx.set_markers(local, pack_ordinal_markers(local, ids[:int(local[-1])]), np.zeros(R, np.uint8), read_begin=0, read_end=half,
                     read_count_total=R, total_marker_count=int(toc[-1]))
     with pytest.raises(capi.ShastaB200Error) as e:
         capi.flag_palindromic_reads(ctx, _params(params))
@@ -179,7 +163,7 @@ def test_facade_writes_read_flags(tmp_path):
     os.makedirs(prefix)
     flags = (np.arange(R) * 5 % 256).astype(np.uint8)
     mm_write_vector(prefix + "Markers.toc", np.asarray(toc, np.uint64))
-    mm_write_vector(prefix + "Markers.data", _data7(toc, ids), object_size=7)
+    mm_write_vector(prefix + "Markers.data", pack_ordinal_markers(toc, ids), object_size=7)
     mm_write_vector(prefix + "ReadFlags", flags)
     a = Assembler(prefix)
     a.accessMarkers()

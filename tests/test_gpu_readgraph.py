@@ -4,19 +4,11 @@ import numpy as np
 import pytest
 
 from oracle import bindings as B
-from shasta_b200 import synth
+from support import ctx, device_alignments  # noqa: F401
 
-from test_oracle_readgraph import _records
+from readgraph_inputs import quality_records, records
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from shasta_b200 import capi
-    c = capi.Context(0)
-    yield c
-    c.close()
 
 
 def _check(ctx, rec, reads, k):
@@ -34,31 +26,23 @@ def test_random_alignment_data(ctx):
     rng = np.random.default_rng(11)
     for n, reads, k in [(0, 5, 3), (1, 4, 6), (60, 12, 3), (5000, 300, 6), (5000, 300, 1), (200, 10, 0), (150, 8, 1000),
                         (200000, 9000, 6)]:
-        _check(ctx, _records(rng, n, reads), reads, k)
+        _check(ctx, records(rng, n, reads), reads, k)
 
 
 def test_on_computed_alignments(ctx):
-    from shasta_b200 import capi
-    d = synth.generate(synth.SynthParams(reads=400, k=10, genome_markers=40000, n50_bases=12000, min_bases=6000, seed=9))
-    kw = dict(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2, maxBucketSize=30, minFrequency=2)
-    ctx.set_markers(d["toc"], d["data"], d["flags"])
-    cand, _, _, _ = ctx.lowhash0(capi.make_lowhash_params(**kw))
-    akw = dict(alignMethod=3, k=10, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=50, minAlignedFraction=0.3,
-               downsamplingFactor=0.1, bandExtend=10, maxBand=1000)
-    rec, _, _, _ = capi.compute_alignments(ctx, cand, capi.make_align_options(**akw))
+    _, _, rec, _, _ = device_alignments(ctx)
     assert len(rec) > 500
     for k in (1, 6, 20):
-        _check(ctx, np.array(rec, np.uint32), 400, k)
+        _check(ctx, rec, 400, k)
 
 
 def test_creation_method_2(ctx):
     """createReadGraph2: thresholds from the histograms (host, alignment order) + the device selection over the alignments that pass."""
     from shasta_b200 import capi
-    from test_oracle_readgraph import _quality_records
     rng = np.random.default_rng(21)
     pc = (0.015, 0.12, 0.12, 0.12, 0.015)
     for n, reads, k in [(0, 4, 6), (400, 30, 6), (3000, 120, 6), (3000, 120, 2), (150000, 6000, 6)]:
-        rec = _quality_records(rng, n, reads)
+        rec = quality_records(rng, n, reads)
         ocrit, orec, okeep, oedges, otoc, odata = B.oracle_create_read_graph2(rec, reads, k, pc)
         work = rec.copy()
         crit, keep, edges, toc, data = capi.create_read_graph2(ctx, work, reads, k, *pc)

@@ -2,27 +2,17 @@
 ReadGraph code (oracle/_ref/libshasta_ref_readgraph_flags.so) where it is built, and otherwise against its outputs recorded in
 tests/golden/reference_readgraph_flags.npz (readgraph_flags_inputs.expected), ties on markerCount included."""
 import os
-import sys
 
 import numpy as np
 import pytest
 
 from oracle import readgraph_flags_bindings as F
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-from readgraph_flags_inputs import DISTANCES, bad_graphs, expected, families, hub  # noqa: E402
+from support import ctx, device_read_graph  # noqa: F401
+from readgraph_flags_inputs import DISTANCES, bad_graphs, expected, families, hub
 
 pytestmark = pytest.mark.gpu
 FAM = families()
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from shasta_b200 import capi
-    c = capi.Context(0)
-    yield c
-    c.close()
 
 
 
@@ -134,27 +124,17 @@ def test_argument_refusals_leave_inputs_unchanged(ctx):
 
 def test_end_to_end_into_marker_graph_vertices(ctx):
     """LowHash0 -> computeAlignments -> createReadGraph2 -> both flags -> createMarkerGraphVertices, all on the device."""
-    from shasta_b200 import capi, synth
+    from shasta_b200 import capi
     from oracle import markergraph_bindings as MB
-    d = synth.generate(synth.SynthParams(reads=400, k=10, genome_markers=40000, n50_bases=12000, min_bases=6000, seed=9))
-    c = capi.Context(0)
-    try:
-        c.set_markers(d["toc"], d["data"], d["flags"])
-        cand, _, _, _ = c.lowhash0(capi.make_lowhash_params(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2,
-                                                           maxBucketSize=30, minFrequency=2))
-        akw = dict(alignMethod=3, k=10, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=50, minAlignedFraction=0.3,
-                   downsamplingFactor=0.1, bandExtend=10, maxBand=1000)
-        rec, ctoc, cdata, _ = capi.compute_alignments(c, cand, capi.make_align_options(**akw))
-        rec = np.array(rec, np.uint32)
-        _, _, edges, toc, data = capi.create_read_graph2(c, rec, 400, 6, 0.015, 0.12, 0.12, 0.12, 0.015)
-        g = dict(edges=np.array(edges), toc=toc, data=data, records=rec.copy(), flags=np.array(d["flags"], np.uint8))
+    with device_read_graph(2) as (c, d, rec, ctoc, cdata, (edges, toc, data)):
+        g = dict(edges=edges, toc=toc, data=data, records=rec.copy(), flags=np.array(d["flags"], np.uint8))
         _check_cross(ctx, "pipeline", g, 6)
         e1, r1, _ = _device_cross(c, g, 6)
         g2 = dict(g, edges=e1, records=r1)
         _check_chimeric(ctx, "pipeline", g2, 2)
         flags, r2, _ = _device_chimeric(c, g2, 2)
         table, vtoc, vdata, hist, res = capi.create_marker_graph_vertices(c, capi.make_marker_graph_params(**MB.DEFAULTS), e1,
-                                                                          np.array(ctoc), np.array(cdata), flags)
+                                                                          ctoc, cdata, flags)
         o = MB.oracle_create_marker_graph_vertices(d["toc"], d["kmer"], e1, ctoc, cdata, flags)
         assert o["status"] == 0
         assert np.array_equal(capi.uint40_to_uint64(table), o["table"]) and np.array_equal(vdata, o["vdata"])
@@ -167,8 +147,6 @@ def test_end_to_end_into_marker_graph_vertices(ctx):
             ref_form = MB.canonical(r["table"], r["vtoc"], r["vdata"])[:3]
             dev_form = MB.canonical(capi.uint40_to_uint64(table), capi.uint40_to_uint64(vtoc), vdata)[:3]
             assert all(np.array_equal(a, b) for a, b in zip(dev_form, ref_form))
-    finally:
-        c.close()
 
 
 def test_facade(tmp_path, monkeypatch, capsys):

@@ -1,6 +1,6 @@
 """GPU (run with -m gpu): shb_create_read_graph, shb_create_read_graph2 (ReadGraph.creationMethod 0 and 2),
 shb_compute_alignment_table and shb_compute_candidate_table against the reference's own code, on the input families of
-tests/test_oracle_readgraph.py, at scale, and on the alignments the device itself computed.
+tests/golden/readgraph_inputs.py, at scale, and on the alignments the device itself computed.
 
 Where oracle/_ref is present with the read graph glue (oracle/ref_glue/ref_readgraph.cpp) the device is compared with it
 directly; elsewhere with the outputs recorded from it in tests/golden/reference_readgraph.npz. Always also with the oracle, which the
@@ -9,21 +9,13 @@ import numpy as np
 import pytest
 
 from oracle import bindings as B
-from shasta_b200 import synth
+from support import assert_same, ctx, device_alignments, outcome, summary, table_summary  # noqa: F401
 
-from test_oracle_readgraph import (DEFAULT_PERCENTILES, assert_same, outcome, read_graph2_families, read_graph_families,
-                                   scale_family, summary, table_summary, unordered2_cases, unordered_cases)
+from readgraph_inputs import (DEFAULT_PERCENTILES, read_graph2_families, read_graph_families, scale_family, unordered2_cases,
+                              unordered_cases)
 from reference_outputs import recorded
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from shasta_b200 import capi
-    c = capi.Context(0)
-    yield c
-    c.close()
 
 
 def _reference(key, fn, *args):
@@ -102,14 +94,7 @@ def test_device_pipeline(ctx):
     reference glue (or, without oracle/_ref, the oracle)."""
     from shasta_b200 import capi
     R = 400
-    d = synth.generate(synth.SynthParams(reads=R, k=10, genome_markers=40000, n50_bases=12000, min_bases=6000, seed=9))
-    kw = dict(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2, maxBucketSize=30, minFrequency=2)
-    ctx.set_markers(d["toc"], d["data"], d["flags"])
-    cand, _, _, _ = ctx.lowhash0(capi.make_lowhash_params(**kw))
-    akw = dict(alignMethod=3, k=10, maxSkip=30, maxDrift=30, maxTrim=30, minAlignedMarkerCount=50, minAlignedFraction=0.3,
-               downsamplingFactor=0.1, bandExtend=10, maxBand=1000)
-    rec, _, _, _ = capi.compute_alignments(ctx, cand, capi.make_align_options(**akw))
-    rec = np.ascontiguousarray(rec, np.uint32)
+    _, cand, rec, _, _ = device_alignments(ctx)
     assert len(rec) > 500
     ref = B.have_ref_readgraph()
     for k in (1, 6, 20):

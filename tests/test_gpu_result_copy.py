@@ -23,11 +23,10 @@ for _path in (HERE, ROOT):                      # run as the subprocess
 
 from oracle import bindings as B  # noqa: E402
 from shasta_b200 import synth  # noqa: E402
+from support import candidate_set, oracle_options  # noqa: E402
 
 OPTS = dict(alignMethod=3, k=14, maxSkip=100, maxDrift=100, maxTrim=100, minAlignedMarkerCount=10, minAlignedFraction=0.1,
             downsamplingFactor=0.05, bandExtend=10, maxBand=1000)
-ALIGN_SET = dict(reads=500, k=14, genome_markers=30000, n50_bases=15000, min_bases=8000, seed=77)
-ALIGN_LOWHASH = dict(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2, maxBucketSize=30, minFrequency=2)
 TILES = 60                                      # 60 x 3000 candidates: 11.5 MB of AlignmentData records at most
 BATCH = 4096
 # LowHash0 on 3000 reads of a 4000-marker genome: every read overlaps hundreds of others, about 2 M candidates (24 MB).
@@ -37,12 +36,9 @@ LOWHASH = dict(m=4, hashFraction=0.01, minHashIterationCount=20, minBucketSize=2
 
 def align_inputs():
     """The markers, the base candidates, and which of them the GPU keeps (from the oracle, so without the GPU)."""
-    d = synth.generate(synth.SynthParams(**ALIGN_SET))
-    lp = B.LowHashParams(**ALIGN_LOWHASH)
-    cand, _, _ = B.oracle_lowhash0(d["toc"], d["data"], d["flags"], lp)
+    d, cand = candidate_set(500, 14, 77, genome_markers=30000)
     base = np.ascontiguousarray(cand[:3000])
-    oo = B.make_align_options(**{k: v for k, v in OPTS.items() if k in B.ALIGN_DEFAULTS})
-    orec, otoc, odata, _ = B.oracle_compute_alignments(d["toc"], d["kmer"], base, oo, threads=8)
+    orec, otoc, odata, _ = B.oracle_compute_alignments(d["toc"], d["kmer"], base, oracle_options(OPTS), threads=8)
     return d, base, orec, otoc, odata
 
 

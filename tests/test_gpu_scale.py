@@ -4,13 +4,11 @@ The production sizes (262 144 candidates per batch, 32 768 jobs per chunk) need 
 seconds, so the library's test hooks SHB_ALIGN_BATCH / SHB_ALIGN_CHUNK shrink them: a few thousand candidates then run through
 many batches, many chunks per band class on all streams, and the result must still be bit-identical to the oracle's and to a
 second run of the same call."""
-import os
-
 import numpy as np
 import pytest
 
 from oracle import bindings as B
-from shasta_b200 import synth
+from support import candidate_set, ctx, oracle_options  # noqa: F401
 
 pytestmark = pytest.mark.gpu
 
@@ -19,37 +17,10 @@ OPTS = dict(alignMethod=3, k=14, maxSkip=100, maxDrift=100, maxTrim=100, minAlig
 
 
 @pytest.fixture(scope="module")
-def ctx():
-    from shasta_b200 import capi
-    c = capi.Context(0)
-    yield c
-    c.close()
-
-
-@pytest.fixture(scope="module")
 def dataset():
-    p = synth.SynthParams(reads=500, k=14, genome_markers=30000, n50_bases=15000, min_bases=8000, seed=77)
-    d = synth.generate(p)
-    lp = B.LowHashParams(m=4, hashFraction=0.01, minHashIterationCount=10, minBucketSize=2, maxBucketSize=30, minFrequency=2)
-    cand, _, _ = B.oracle_lowhash0(d["toc"], d["data"], d["flags"], lp)
+    d, cand = candidate_set(500, 14, 77, genome_markers=30000)
     assert len(cand) > 2500
     return d, cand[:3000]
-
-
-class _Hooks:
-    def __init__(self, **env):
-        self.env = env
-
-    def __enter__(self):
-        self.saved = {k: os.environ.get(k) for k in self.env}
-        os.environ.update({k: str(v) for k, v in self.env.items()})
-
-    def __exit__(self, *exc):
-        for k, v in self.saved.items():
-            if v is None:
-                os.environ.pop(k, None)
-            else:
-                os.environ[k] = v
 
 
 def _run(ctx, d, cand, **opts):
@@ -60,49 +31,53 @@ def _run(ctx, d, cand, **opts):
 
 
 @pytest.mark.parametrize("batch,chunk", [(700, 64), (257, 1000000), (4096, 33)])
-def test_small_batches_and_chunks_match_oracle(ctx, dataset, batch, chunk):
+def test_small_batches_and_chunks_match_oracle(ctx, dataset, monkeypatch, batch, chunk):
     d, cand = dataset
-    oo = B.make_align_options(**{k: v for k, v in OPTS.items() if k in B.ALIGN_DEFAULTS})
-    orec, otoc, odata, _ = B.oracle_compute_alignments(d["toc"], d["kmer"], cand, oo, threads=8)
-    with _Hooks(SHB_ALIGN_BATCH=batch, SHB_ALIGN_CHUNK=chunk):
-        rec, ctoc, cdata, res = _run(ctx, d, cand, **OPTS)
+    orec, otoc, odata, _ = B.oracle_compute_alignments(d["toc"], d["kmer"], cand, oracle_options(OPTS), threads=8)
+    monkeypatch.setenv("SHB_ALIGN_BATCH", str(batch))
+    monkeypatch.setenv("SHB_ALIGN_CHUNK", str(chunk))
+    rec, ctoc, cdata, res = _run(ctx, d, cand, **OPTS)
     assert res.candidateCount == len(cand)
     assert len(orec) > 300
     assert np.array_equal(rec, orec) and np.array_equal(ctoc, otoc) and np.array_equal(cdata, odata)
 
 
 @pytest.mark.parametrize("workers", [1, 2, 3])
-def test_worker_threads_match_oracle(ctx, dataset, workers):
+def test_worker_threads_match_oracle(ctx, dataset, monkeypatch, workers):
     # The batches of one call are spread over host worker threads, each with its own streams and scratch; the kept
     # alignments land in a shared arena in completion order and are put back into candidate order at the end.
     d, cand = dataset
-    oo = B.make_align_options(**{k: v for k, v in OPTS.items() if k in B.ALIGN_DEFAULTS})
-    orec, otoc, odata, _ = B.oracle_compute_alignments(d["toc"], d["kmer"], cand, oo, threads=8)
-    with _Hooks(SHB_ALIGN_BATCH=211, SHB_ALIGN_CHUNK=70, SHB_ALIGN_WORKERS=workers):
-        for _ in range(2):
-            rec, ctoc, cdata, res = _run(ctx, d, cand, **OPTS)
-            assert res.workers == workers
-            assert np.array_equal(rec, orec) and np.array_equal(ctoc, otoc) and np.array_equal(cdata, odata)
+    orec, otoc, odata, _ = B.oracle_compute_alignments(d["toc"], d["kmer"], cand, oracle_options(OPTS), threads=8)
+    monkeypatch.setenv("SHB_ALIGN_BATCH", "211")
+    monkeypatch.setenv("SHB_ALIGN_CHUNK", "70")
+    monkeypatch.setenv("SHB_ALIGN_WORKERS", str(workers))
+    for _ in range(2):
+        rec, ctoc, cdata, res = _run(ctx, d, cand, **OPTS)
+        assert res.workers == workers
+        assert np.array_equal(rec, orec) and np.array_equal(ctoc, otoc) and np.array_equal(cdata, odata)
 
 
-def test_method4_small_batches_match_oracle(ctx, dataset):
+def test_method4_small_batches_match_oracle(ctx, dataset, monkeypatch):
     d, cand = dataset
     opts = dict(OPTS, alignMethod=4)
-    oo = B.make_align_options(**{k: v for k, v in opts.items() if k in B.ALIGN_DEFAULTS})
-    orec, otoc, odata, _ = B.oracle_compute_alignments(d["toc"], d["kmer"], cand[:1200], oo, threads=8)
-    with _Hooks(SHB_ALIGN_BATCH=300, SHB_ALIGN_CHUNK=50):
-        rec, ctoc, cdata, _ = _run(ctx, d, cand[:1200], **opts)
+    orec, otoc, odata, _ = B.oracle_compute_alignments(d["toc"], d["kmer"], cand[:1200], oracle_options(opts), threads=8)
+    monkeypatch.setenv("SHB_ALIGN_BATCH", "300")
+    monkeypatch.setenv("SHB_ALIGN_CHUNK", "50")
+    rec, ctoc, cdata, _ = _run(ctx, d, cand[:1200], **opts)
     assert np.array_equal(rec, orec) and np.array_equal(ctoc, otoc) and np.array_equal(cdata, odata)
 
 
-def test_repeated_calls_are_identical(ctx, dataset):
+def test_repeated_calls_are_identical(ctx, dataset, monkeypatch):
     # The chunks of a batch run on several streams; a missing dependency would show up as run-to-run differences.
     d, cand = dataset
-    with _Hooks(SHB_ALIGN_BATCH=1500, SHB_ALIGN_CHUNK=100):
-        first = _run(ctx, d, cand, **OPTS)
-        for _ in range(3):
-            again = _run(ctx, d, cand, **OPTS)
-            assert all(np.array_equal(x, y) for x, y in zip(first[:3], again[:3]))
+    monkeypatch.setenv("SHB_ALIGN_BATCH", "1500")
+    monkeypatch.setenv("SHB_ALIGN_CHUNK", "100")
+    first = _run(ctx, d, cand, **OPTS)
+    for _ in range(3):
+        again = _run(ctx, d, cand, **OPTS)
+        assert all(np.array_equal(x, y) for x, y in zip(first[:3], again[:3]))
     # ... and the production sizes give the same answer as the shrunken ones
+    monkeypatch.delenv("SHB_ALIGN_BATCH")
+    monkeypatch.delenv("SHB_ALIGN_CHUNK")
     full = _run(ctx, d, cand, **OPTS)
     assert all(np.array_equal(x, y) for x, y in zip(first[:3], full[:3]))

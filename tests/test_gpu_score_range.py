@@ -40,25 +40,24 @@ ROOT = os.path.dirname(HERE)
 sys.path.insert(0, ROOT)
 
 import bench  # noqa: E402
-import test_gpu_align_limits as AL  # noqa: E402
-import test_gpu_configs as CFG  # noqa: E402
 from oracle import bindings as B  # noqa: E402
+from support import (CONFIGS, FORWARD_MAX_MARKERS, FORWARD_MAX_ROWS, K, MAX_BAND_WIDTH, PERMISSIVE, assemble,  # noqa: E402,F401
+                     compare_alignments, ctx, downsampled, downsampling_hash, downsampling_threshold, expected_single_pair,
+                     padded_width, single_pair_options, wide_band_class)
 
-K = AL.K
 SCORE_LIMIT = 1 << 28
 NEG_INF, GAP_BARRIER, END_NONE = -(1 << 29), -(1 << 28), -(1 << 30)     # kNegInf, kGapBarrier, kNegInf * 2
 INT32 = (-(1 << 31), (1 << 31) - 1)
 DROP_FACTOR = 0.5           # tails and runs use k-mers this downsampling (and every smaller factor) drops
-FORWARD_MAX_ROWS, FORWARD_MAX_MARKERS = AL.FORWARD_MAX_ROWS, AL.FORWARD_MAX_MARKERS
 
 
 def in_bound(m, longest):
-    return m * (2 * longest + AL.MAX_BAND_WIDTH) < SCORE_LIMIT
+    return m * (2 * longest + MAX_BAND_WIDTH) < SCORE_LIMIT
 
 
 def largest_score(longest):
     """The largest M the bound admits for reads of up to `longest` markers."""
-    return (SCORE_LIMIT - 1) // (2 * longest + AL.MAX_BAND_WIDTH)
+    return (SCORE_LIMIT - 1) // (2 * longest + MAX_BAND_WIDTH)
 
 
 def score_opts(m):
@@ -129,8 +128,8 @@ def band_shape(lo, hi):
     """(lanes, c, padded width) of a band (dpBandShape); c = 0 is the scan kernel."""
     need = hi - lo + 3
     if need <= 128:
-        return 8, max(2, -(-need // 16)), AL.padded_width(hi - lo + 1)
-    return 32, next((c for c in (3, 4, 6, 8, 12, 16) if need <= 64 * c), 0), AL.padded_width(hi - lo + 1)
+        return 8, max(2, -(-need // 16)), padded_width(hi - lo + 1)
+    return 32, next((c for c in (3, 4, 6, 8, 12, 16) if need <= 64 * c), 0), padded_width(hi - lo + 1)
 
 
 def _row_kmers(b, j):
@@ -297,16 +296,16 @@ class Pool:
     def take(self, n, dropped=False):
         ok = ~self.used
         if dropped:
-            ok &= AL.downsampling_hash(self.ids, K) >= np.uint32(int(DROP_FACTOR * 4294967295.0))
+            ok &= downsampling_hash(self.ids, K) >= downsampling_threshold(DROP_FACTOR)
         pick = np.flatnonzero(ok)[:n]
         assert len(pick) == n
         self.used[pick] = True
         return self.ids[pick]
 
 
-M3 = dict(AL.PERMISSIVE, alignMethod=3, downsamplingFactor=0.1, bandExtend=10, maxBand=1000)
+M3 = dict(PERMISSIVE, alignMethod=3, downsamplingFactor=0.1, bandExtend=10, maxBand=1000)
 M3_TRACED = dict(M3, downsamplingFactor=DROP_FACTOR, bandExtend=200)
-M1 = dict(AL.PERMISSIVE, alignMethod=1)
+M1 = dict(PERMISSIVE, alignMethod=1)
 WIDE_EXTEND, WIDE_MAX_BAND = 8158, 16317
 
 
@@ -350,11 +349,6 @@ def longest(name):
 
 def family_scores(name):
     return score_opts(largest_score(longest(name)))
-
-
-def downsampled(row, factor):
-    keep = np.flatnonzero(AL.downsampling_hash(row, K) < np.uint32(int(factor * 4294967295.0)))
-    return row[keep], keep.astype(np.int64)
 
 
 def dp_problems(a, b, opts, sc):
@@ -461,11 +455,11 @@ def test_scan_kernel_wraps_far_beyond_the_bound():
 
 
 def test_shipped_configurations_sit_far_inside_the_bound():
-    sets = [dict(B.ALIGN_DEFAULTS, **cfg["align"]) for cfg in CFG.CONFIGS.values()] + [dict(bench.ALIGN_DEFAULT)]
+    sets = [dict(B.ALIGN_DEFAULTS, **cfg["align"]) for cfg in CONFIGS.values()] + [dict(bench.ALIGN_DEFAULT)]
     for o in sets:
         m = 6 if o["alignMethod"] == 4 else max(abs(o["matchScore"]), abs(o["mismatchScore"]), abs(o["gapScore"]))
         assert m == 6
-        assert 5 * m * (2 * 4_000_000 + AL.MAX_BAND_WIDTH) < SCORE_LIMIT        # reads of 4 M markers, 5x margin
+        assert 5 * m * (2 * 4_000_000 + MAX_BAND_WIDTH) < SCORE_LIMIT        # reads of 4 M markers, 5x margin
         assert in_bound(m, (1 << 24) - 1)                                        # every read the reference can store
     assert largest_score(4_000_000) >= 30
 
@@ -499,28 +493,20 @@ def test_cases_reach_their_paths():
             assert len(stage2) == 8 and (True, False) in sides and (False, True) in sides
         if name == "widest":
             assert sorted(widths)[-2:] == [WIDE_MAX_BAND, 16381]
-            assert AL._class_of(16381) == AL._class_of(WIDE_MAX_BAND) == 16384
+            assert wide_band_class(16381) == wide_band_class(WIDE_MAX_BAND) == 16384
     assert {(1, "method1"), (3, "forward"), (3, "traced"), (3, "stage2")} <= kinds
     assert {("method1", 8), ("method1", 32), ("method1", "scan"), ("stage2", 8), ("stage2", 32), ("stage2", "scan"),
             ("traced", "scan")} <= classes
 
 
 # ---- GPU tests ---------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def ctx():
-    from shasta_b200 import capi
-    c = capi.Context(0)
-    yield c
-    c.close()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", FAMILIES)
 def test_device_matches_oracle_at_the_bound(ctx, name):
     rows, cand, opts = family(name)
-    d = AL.assemble(rows)
+    d = assemble(rows, K)
     for o in opts:
-        AL.compare(ctx, d, cand, **o, **family_scores(name))
+        compare_alignments(ctx, d, cand, **o, **family_scores(name))
 
 
 @pytest.mark.gpu
@@ -528,7 +514,7 @@ def test_device_matches_oracle_at_the_bound(ctx, name):
 def test_single_pair_at_the_bound(ctx, name):
     from shasta_b200 import capi
     rows, cand, opts = family(name)
-    d = AL.assemble(rows)
+    d = assemble(rows, K)
     ctx.set_markers(d["toc"], d["data"], d["flags"])
     stored = 0
     for o in opts:
@@ -537,7 +523,7 @@ def test_single_pair_at_the_bound(ctx, name):
         for r0, r1, _ in cand:
             for o0, o1 in ((2 * int(r0), 2 * int(r1)), (2 * int(r1), 2 * int(r0))):
                 ords, info = capi.align_oriented_reads(ctx, o0, o1, go)
-                exp = AL.expected_single_pair(rows[o0 // 2], rows[o1 // 2], o)
+                exp = expected_single_pair(rows[o0 // 2], rows[o1 // 2], o)
                 if exp is None:
                     assert len(ords) == 0 and not info.any(), (o0, o1)
                     continue
@@ -552,7 +538,7 @@ def test_single_pair_at_the_bound(ctx, name):
 def test_refused_beyond_the_bound(ctx, name):
     from shasta_b200 import capi
     rows, cand, opts = family(name)
-    d = AL.assemble(rows)
+    d = assemble(rows, K)
     ctx.set_markers(d["toc"], d["data"], d["flags"])
     m = largest_score(longest(name)) + 1
     for o in opts:
@@ -567,9 +553,9 @@ def test_refused_beyond_the_bound(ctx, name):
     if len(cand) > 1:
         short = max(len(rows[int(cand[0, 0])]), len(rows[int(cand[0, 1])]))
         assert in_bound(m, short)
-        AL.compare(ctx, d, cand[:1], **opts[0], **score_opts(m))
+        compare_alignments(ctx, d, cand[:1], **opts[0], **score_opts(m))
     # Align4 scores 6/-1/-1 whatever the options say: never refused for them, and bit-exact with the oracle's Align4,
     # which hard-codes those scores too.
-    AL.compare(ctx, d, cand, **dict(AL.single_pair_options(4), **score_opts(m)))
+    compare_alignments(ctx, d, cand, **dict(single_pair_options(4), **score_opts(m)))
     # The same context then aligns in range, bit-exact.
-    AL.compare(ctx, d, cand, **opts[-1], **family_scores(name))
+    compare_alignments(ctx, d, cand, **opts[-1], **family_scores(name))

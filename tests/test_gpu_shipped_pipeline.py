@@ -9,7 +9,6 @@ edges, and at k = 8 some marker set holds two markers of one read and a read ali
 has a k-mer at exactly maxMarkerFrequency. The Align4 grid path (more than 512 existing cells) is not reached by these inputs:
 the count of such candidates is printed, and tests/test_gpu_align.py reaches the path through SHB_ALIGN4_SMEM_CELLS."""
 import os
-import sys
 import time
 
 import numpy as np
@@ -21,9 +20,9 @@ from oracle import markergraph_edges_bindings as EB
 from oracle import palindromic_bindings as PB
 from oracle import readgraph_flags_bindings as F
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
-import pipeline_inputs as P  # noqa: E402
-import pipeline_reference as T  # noqa: E402
+import support  # noqa: F401  (puts tests/golden on sys.path)
+import pipeline_inputs as P
+import pipeline_reference as T
 
 pytestmark = pytest.mark.gpu
 NAMES = list(P.CONFIGS)

@@ -4,15 +4,9 @@ chains), skewed digits, one and two bit ranges, with and without a payload, repe
 import numpy as np
 import pytest
 
+from support import ctx  # noqa: F401
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def ctx():
-    from shasta_b200 import capi
-    c = capi.Context(0)
-    yield c
-    c.close()
 
 
 def _sort(ctx, keys, vals, lo, hi):

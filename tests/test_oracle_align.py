@@ -9,16 +9,14 @@ The overlap DP's tie-break rule is 'parity unpinned' (SeqAn absent, SURVEY.md F4
   * DP optimality properties that hold for any correct implementation (score = brute force, path validity).
 """
 import ctypes as C
-import os
-import sys
 
 import numpy as np
 
 from oracle import bindings as B
 from shasta_b200 import synth
+from support import downsampling_hash
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
-from reference_outputs import recorded  # noqa: E402
+from reference_outputs import recorded
 
 # src/compressAlignment.cpp:161-192 (testAlignmentCompression): 30 ordinal pairs exercising Formats 0-4.
 COMPRESSION_TEST_VECTOR = [
@@ -67,14 +65,13 @@ def _ref_murmurhash2_u64(n):
 def test_downsampling_hash_at_k16():
     # At k = 16 the sum n = kmerId + rc(kmerId) can reach 2^32, so the second word of the 8-byte MurmurHash2 is not zero
     # (src/AssemblerKmers.cpp:182-186): the oracle's hash and the tests' numpy model against the reference's MurmurHash2 of n.
-    import test_gpu_align_limits as AL
     ids = np.random.default_rng(16).integers(0, 1 << 32, 100000, dtype=np.uint64).astype(np.uint32)
     n = ids.astype(np.uint64) + synth.reverse_complement_kmer(ids, 16).astype(np.uint64)
     assert (n >> np.uint64(32) != 0).sum() > 40000
     expected = recorded("align", "downsampling_hash_k16", _ref_murmurhash2_u64, n)
     lib = B.oracle_lib()
     assert np.array_equal(np.array([lib.orc_kmer_downsampling_hash(x, 16) for x in ids.tolist()], np.uint32), expected)
-    assert np.array_equal(AL.downsampling_hash(ids, 16), expected)
+    assert np.array_equal(downsampling_hash(ids, 16), expected)
 
 
 def _brute_score(a, b, match, mismatch, gap, band=None):

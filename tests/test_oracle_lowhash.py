@@ -7,7 +7,6 @@ Golden material (SURVEY.md section 8c / Appendix B, D):
 """
 import json
 import os
-import sys
 
 import numpy as np
 import pytest
@@ -15,9 +14,9 @@ import pytest
 from oracle import bindings as B
 from shasta_b200 import synth
 
-sys.path.insert(0, os.path.join(os.path.dirname(__file__), "golden"))
-import make_golden as MG  # noqa: E402
-from reference_outputs import recorded  # noqa: E402
+import support  # noqa: F401  (puts tests/golden on sys.path)
+import make_golden as MG
+from reference_outputs import recorded
 
 
 def test_murmurhash64a_known_answers():

@@ -3,18 +3,14 @@ against the reference's own DisjointSets, decompress and PeakFinder driven in th
 (oracle/ref_glue/ref_markergraph.cpp), in canonical form (vertices by first marker). PeakFinder alone: the library's
 restatement (shb_peak_finder_cutoff) and the oracle's against the reference on a few hundred histograms. The reference's
 outputs are stored in tests/golden/reference_markergraph.npz."""
-import hashlib
-import os
-import sys
-
 import numpy as np
 import pytest
 
 from oracle import markergraph_bindings as MB
+import support  # noqa: F401  (tests/golden on sys.path)
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
-from markergraph_inputs import PARAMS, START_INDEX, cases, histograms  # noqa: E402
-from reference_outputs import recorded  # noqa: E402
+from markergraph_inputs import PARAMS, START_INDEX, cases, histograms
+from reference_outputs import recorded, shrink
 
 CASES = cases()
 HISTOGRAMS = histograms()
@@ -51,18 +47,12 @@ def test_peak_finder():
 
 def pack(table, vtoc, vdata):
     """Canonical vertices in a form that compresses: table as marker id minus first marker (2^40-1 kept), vertex sizes,
-    and the differences of consecutive vertex markers."""
+    and the differences of consecutive vertex markers. Arrays of the long-read case are stored as their SHA-256."""
     table = np.asarray(table, np.uint64)
     inv = np.uint64((1 << 40) - 1)
     delta = np.where(table == inv, inv, np.arange(len(table), dtype=np.uint64) - table)
     out = dict(table=delta, sizes=np.diff(np.asarray(vtoc, np.uint64)), steps=np.diff(np.asarray(vdata, np.uint64), prepend=np.uint64(0)))
-    return {k: shrink(v) for k, v in out.items()}
-
-
-def shrink(a):
-    """Arrays of the long-read case are stored as their SHA-256."""
-    a = np.ascontiguousarray(a, np.uint64)
-    return np.frombuffer(hashlib.sha256(a.tobytes()).digest(), np.uint8) if len(a) > 50_000 else a
+    return {k: shrink(np.asarray(v, np.uint64), 50_000) for k, v in out.items()}
 
 
 def _ref_case(name, pname):
@@ -78,7 +68,7 @@ def _ref_case(name, pname):
     crc[rank] = rank[rc.astype(np.int64)]
     keys = ("histogram", "minCoverageUsed", "peakFinderFailed", "disjointSetCount", "keptDisjointSetCount",
             "badDisjointSetCount", "vertexCount", "observedAreaFraction")
-    return dict(rc=shrink(crc), **pack(table, vtoc, vdata), **{k: r[k] for k in keys})
+    return dict(rc=shrink(np.asarray(crc, np.uint64), 50_000), **pack(table, vtoc, vdata), **{k: r[k] for k in keys})
 
 
 @pytest.mark.parametrize("pname", sorted(PARAMS))
@@ -97,7 +87,7 @@ def test_oracle_equals_reference(name, pname):
                 "vertexCount", "observedAreaFraction"):
         assert o[key] == ref[key], key
     st, rc = MB.oracle_find_rc_vertices(d["toc"], o["table"], o["vtoc"], o["vdata"])
-    assert st == 0 and np.array_equal(shrink(rc), np.asarray(ref["rc"]).reshape(-1))
+    assert st == 0 and np.array_equal(shrink(np.asarray(rc, np.uint64), 50_000), np.asarray(ref["rc"]).reshape(-1))
     assert o["edgePairsUsed"] + o["edgePairsSkipped"] == len(d["edges"]) // 2
 
 

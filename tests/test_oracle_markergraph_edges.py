@@ -7,24 +7,18 @@ each with a digest of its input; arrays above 4096 elements as their SHA-256."""
 import ctypes as C
 import os
 import subprocess
-import sys
 
 import numpy as np
 import pytest
 
 from oracle import markergraph_edges_bindings as EB
+import support  # noqa: F401  (tests/golden on sys.path)
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
-from markergraph_edges_inputs import digest, vertex_cases  # noqa: E402
-from reference_outputs import recorded  # noqa: E402
+from markergraph_edges_inputs import digest, rc_failure_inputs, vertex_cases
+from reference_outputs import recorded, shrink
 
 CASES = vertex_cases()
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def shrink(a):
-    a = np.ascontiguousarray(a)
-    return np.frombuffer(__import__("hashlib").sha256(a.tobytes()).digest(), np.uint8) if a.size > 4096 else a
 
 
 def exact_form(s):
@@ -49,23 +43,23 @@ def _ref_case(name):
     d = CASES[name]
     one = EB.ref_create_marker_graph_edges(d["toc"], d["table"], d["vtoc"], d["vdata"], threads=1)
     assert one["status"] == 0
-    out = {f"one/{k}": shrink(v) for k, v in exact_form(one).items()}
+    out = {f"one/{k}": shrink(v, 4096) for k, v in exact_form(one).items()}
     many = EB.ref_create_marker_graph_edges(d["toc"], d["table"], d["vtoc"], d["vdata"], threads=0)
     rc_many = None
     if d["rc"] is not None:
         msg, rc = EB.ref_find_rc_edges(d["toc"], d["rc"], one, threads=1)
         out["rc_message"] = msg or ""
-        out["one/rc"] = shrink(rc if rc is not None else np.zeros(0, np.uint64))
+        out["one/rc"] = shrink(rc if rc is not None else np.zeros(0, np.uint64), 4096)
         msg_many, rc_many = EB.ref_find_rc_edges(d["toc"], d["rc"], many, threads=0)
         assert msg_many == msg or (msg and msg_many)
-    out.update({f"all/{k}": shrink(v) for k, v in canonical_form(many, rc_many).items()})
+    out.update({f"all/{k}": shrink(v, 4096) for k, v in canonical_form(many, rc_many).items()})
     out["input"] = _input_digest(d)
     return out
 
 
 def _check(got, ref, prefix):
     for k, v in got.items():
-        assert np.array_equal(shrink(v).reshape(-1), np.asarray(ref[f"{prefix}/{k}"]).reshape(-1)), f"{prefix}/{k}"
+        assert np.array_equal(shrink(v, 4096).reshape(-1), np.asarray(ref[f"{prefix}/{k}"]).reshape(-1)), f"{prefix}/{k}"
 
 
 @pytest.mark.parametrize("name", sorted(CASES))
@@ -81,7 +75,7 @@ def test_oracle_equals_reference(name):
         msg, rc = EB.oracle_find_rc_edges(d["toc"], d["rc"], o)
         assert (msg or "") == ref["rc_message"]
         if rc is not None:
-            assert np.array_equal(shrink(rc).reshape(-1), np.asarray(ref["one/rc"]).reshape(-1))
+            assert np.array_equal(shrink(rc, 4096).reshape(-1), np.asarray(ref["one/rc"]).reshape(-1))
     _check(canonical_form(o, rc), ref, "all")
 
 
@@ -109,49 +103,15 @@ def test_cases_reach_every_branch():
     assert {"self_loop", "saturated", "zero", "long_gap", "permuted"} <= seen
 
 
-def _parallel(s, e):
-    """Edge e duplicated at the end of the edge list, with its intervals, and listed in its source's row: parallel edges."""
-    s = {k: np.array(v) for k, v in s.items() if isinstance(v, np.ndarray)}
-    E = len(s["edges"])
-    itoc = s["intervalsToc"].astype(np.int64)
-    s["edges"] = np.concatenate([s["edges"], s["edges"][e:e + 1]])
-    s["intervalsData"] = np.concatenate([s["intervalsData"], s["intervalsData"][itoc[e]:itoc[e + 1]]])
-    s["intervalsToc"] = np.append(s["intervalsToc"], s["intervalsToc"][-1] + (itoc[e + 1] - itoc[e])).astype(np.uint64)
-    src = int(EB.named_fields(s["edges"][e:e + 1])[0, 0])
-    stoc = s["bySourceToc"].astype(np.int64)
-    data = list(s["bySourceData"].tolist())
-    data.insert(stoc[src], E)                            # the new id first: rows are in decreasing edge id
-    s["bySourceData"] = np.array(data, np.uint64)
-    s["bySourceToc"][src + 1:] += 1
-    return s
-
-
-def _drop_interval(s, e):
-    s = {k: np.array(v) for k, v in s.items() if isinstance(v, np.ndarray)}
-    itoc = s["intervalsToc"].astype(np.int64)
-    s["intervalsData"] = np.delete(s["intervalsData"], itoc[e + 1] - 1, axis=0)
-    s["intervalsToc"][e + 1:] -= 1
-    return s
-
-
-def rc_failure_inputs():
-    """(name, vertices, edge set) for the two failures the reference reports."""
-    d = CASES["genome/cov2"]
-    o = EB.oracle_create_marker_graph_edges(d["toc"], d["table"], d["vtoc"], d["vdata"])
-    cov = np.diff(o["intervalsToc"].astype(np.int64))
-    e = int(np.nonzero(cov >= 2)[0][3])
-    return [("missing_interval", d, _drop_interval(o, e)), ("parallel", d, _parallel(o, e))]
-
-
 def _ref_rc_failure(i):
-    name, d, s = rc_failure_inputs()[i]
+    name, d, s = rc_failure_inputs(CASES["genome/cov2"])[i]
     msg, _ = EB.ref_find_rc_edges(d["toc"], d["rc"], s, threads=1)
     return dict(message=msg or "", input=digest(s["edges"], s["intervalsToc"], s["intervalsData"], s["bySourceToc"], s["bySourceData"]))
 
 
 @pytest.mark.parametrize("i", [0, 1])
 def test_rc_failures_give_the_reference_messages(i):
-    name, d, s = rc_failure_inputs()[i]
+    name, d, s = rc_failure_inputs(CASES["genome/cov2"])[i]
     ref = recorded("markergraph_edges", f"rc_failure/{name}", _ref_rc_failure, i)
     assert np.array_equal(ref["input"], digest(s["edges"], s["intervalsToc"], s["intervalsData"], s["bySourceToc"], s["bySourceData"]))
     msg, rc = EB.oracle_find_rc_edges(d["toc"], d["rc"], s)

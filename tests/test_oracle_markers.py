@@ -3,15 +3,13 @@ MarkerFinder on TinyTest (tests/golden/tinytest_markers.npz; inputs tests/golden
 reference's ReadLoader + MarkerFinder run on synthetic FASTA files (recorded in tests/golden/reference_markers.npz)."""
 import hashlib
 import os
-import sys
 
 import numpy as np
 
 from oracle import bindings as B
+from support import reference_markers
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
-from reference_outputs import recorded  # noqa: E402
 
 # (reads, seed, k) of the synthetic FASTA files: this test's, then the GPU test's (tests/test_gpu_markers.py)
 SYNTHETIC_CASES = [(40, 3, 8), (40, 3, 10), (60, 6, 6), (60, 10, 10), (60, 14, 14)]
@@ -30,33 +28,6 @@ def test_marker_oracle_reproduces_reference_tinytest():
     toc, data = B.oracle_find_markers(r["word_offsets"], r["words"], r["base_counts"], is_marker, 10)
     assert toc[-1] == 124036                    # SURVEY.md F5
     assert np.array_equal(toc, m["toc"]) and np.array_equal(data, m["data"])
-
-
-def write_synthetic_fasta(path, reads=40, seed=3):
-    rng = np.random.default_rng(seed)
-    with open(path, "w") as f:
-        for i in range(reads):
-            n = int(rng.integers(10000, 14000))
-            # homopolymer runs of random length so that the run-length encoding has something to do
-            bases = np.repeat(rng.integers(0, 4, n), rng.integers(1, 4, n))[:n]
-            f.write(f">read{i}\n" + "".join("ACGT"[b] for b in bases) + "\n")
-
-
-def _reference_markers(path, reads, seed, k):
-    write_synthetic_fasta(path, reads=reads, seed=seed)
-    r = B.ref_reads_from_fasta(path, k=k, min_read_length=1000)
-    m = B.ref_markers_from_fasta(path, k=k, min_read_length=1000)
-    # The marker table is stored as the marker k-mers that occur (both strands): k-mers absent from the reads cannot change
-    # the output, and the whole table is 4^k entries. The 7-byte records are stored as their SHA-256.
-    kmers = np.ascontiguousarray(m["data"].reshape(-1, 7)[:, :4]).view("<u4").reshape(-1)
-    return dict(word_offsets=r["word_offsets"], words=r["words"], base_counts=r["base_counts"], marker_kmers=np.unique(kmers),
-                toc=m["toc"], flags=m["flags"], data_sha256=hashlib.sha256(m["data"].tobytes()).hexdigest())
-
-
-def reference_markers(tmp_path, reads, seed, k):
-    """What the reference's ReadLoader and MarkerFinder make of write_synthetic_fasta(reads, seed) with k-mer length k."""
-    return recorded("markers", f"reads{reads}_seed{seed}_k{k}", _reference_markers, str(tmp_path / f"synthetic_{seed}.fasta"),
-                    reads, seed, k)
 
 
 def test_marker_oracle_against_live_reference(tmp_path):

@@ -1,17 +1,14 @@
 """flagPalindromicReads: the C restatement (oracle/palindromic_oracle.c) against the unmodified reference build
 (shasta::align of src/AlignmentGraph.cpp and the thresholds of src/AssemblerAlign.cpp:741-766), read for read and path
 for path. The reference's outputs are stored in tests/golden/reference_palindromic.npz."""
-import os
-import sys
-
 import numpy as np
 import pytest
 
 from oracle import palindromic_bindings as B
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
-from palindromic_inputs import cases, killer_case  # noqa: E402
-from reference_outputs import recorded  # noqa: E402
+import support  # noqa: F401  (puts tests/golden on sys.path)
+from palindromic_inputs import cases, killer_case
+from reference_outputs import recorded
 
 CASES = cases()
 

@@ -1,16 +1,13 @@
 """flagCrossStrandReadGraphEdges1 and flagChimericReads: the restatement in oracle/readgraph_flags_bindings.py against the
 reference's own ReadGraph code (oracle/_ref/libshasta_ref_readgraph_flags.so) on read graphs built directly. Where that
 build is absent the comparisons use its outputs recorded in tests/golden/reference_readgraph_flags.npz."""
-import os
-import sys
-
 import numpy as np
 import pytest
 
 from oracle import readgraph_flags_bindings as F
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
-from readgraph_flags_inputs import DISTANCES, bad_graphs, expected, families, hub  # noqa: E402
+import support  # noqa: F401  (puts tests/golden on sys.path)
+from readgraph_flags_inputs import DISTANCES, bad_graphs, expected, families, hub
 
 FAM = families()
 need_ref = pytest.mark.skipif(not F.have_ref(), reason="the reference build oracle/_ref/libshasta_ref_readgraph_flags.so is absent")

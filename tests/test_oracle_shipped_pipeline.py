@@ -8,9 +8,6 @@ flagChimericReads, createMarkerGraphVertices, findMarkerGraphReverseComplementVe
 findMarkerGraphReverseComplementEdges; for computeAlignments the reference's AlignmentInfo and compressAlignment check every
 stored record and its compressed bytes (the DP itself is the oracle's: SeqAn is absent). Markers at k 8 and 15 are
 oracle-only."""
-import os
-import sys
-
 import numpy as np
 import pytest
 
@@ -20,10 +17,10 @@ from oracle import markergraph_edges_bindings as EB
 from oracle import palindromic_bindings as PB
 from oracle import readgraph_flags_bindings as F
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
-import pipeline_inputs as P  # noqa: E402
-import pipeline_reference as PR  # noqa: E402
-from pipeline_reference import reference, same  # noqa: E402
+import support  # noqa: F401  (puts tests/golden on sys.path)
+import pipeline_inputs as P
+import pipeline_reference as PR
+from pipeline_reference import reference, same
 
 NAMES = list(P.CONFIGS)
 

@@ -1,14 +1,11 @@
 """ReadLowHashStatistics.csv written by the facade against the file the reference's own LowHash0 leaves in its working directory
 (src/LowHash0.cpp:220-243), recorded in tests/golden/reference_csv.npz."""
-import os
-import sys
-
 from oracle import bindings as B
 from shasta_b200 import assembler as A
 from shasta_b200 import synth
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden"))
-from reference_outputs import recorded  # noqa: E402
+import support  # noqa: F401  (puts tests/golden on sys.path)
+from reference_outputs import recorded
 
 
 def _reference_csv(d, p):
